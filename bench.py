@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- the headline benchmark of BASELINE.json: AGD iters/sec & examples/sec on logistic
-10M x 1024 dense fp32 (configs[1]), 1/2/4/8 B200, next to the reference's path on the host cores.
+10M x 1024 dense fp32 (configs[1]), 1/2/4/8 H100, next to the reference's path on the host cores.
 
   python bench.py --gpus N --steps K --warmup W            (N > 1: launched under torchrun, one rank per GPU)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py ... --dump-outputs DIR                   (rank 0 writes the timed run's weights and loss history)
 
 A "step" is one outer AGD iteration (AGD.scala:237-332) = the reference's 3 + 2b applySmooth evaluations
 (flags = 0: every evaluation is executed; the history evaluation of :304 shares one sweep over X with the next
@@ -51,12 +52,14 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-rows", type=int, default=0, help="rows of the bounded CPU sample (0 = 4M, the same at every N)")
     ap.add_argument("--store", default="f32", choices=["f32", "bf16", "f64"],
-                    help="HBM storage of the logistic_f32 workload; bf16 is the stated substitute that lets the 100M x 512 "
-                         "shape of configs[4] fit ONE GPU (204.8 GB as fp32); f64 is what the Scala facade stores by default "
-                         "(arbitrary Double features kept exact)")
+                    help="HBM storage of the logistic_f32 workload; bf16 halves the bytes per row (the 100M x 512 shape of "
+                         "configs[4] is 204.8 GB as fp32, 102.4 GB as bf16: two or more 80 GB GPUs either way); f64 is what "
+                         "the Scala facade stores by default (arbitrary Double features kept exact)")
     ap.add_argument("--parity-iters", type=int, default=10,
                     help="iterations of the full-size oracle comparison reported as `parity` (0 = off; on by default for "
                          "fp32 logistic workloads whose host copy is <= 64 GB)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed run returned (weights, loss history) as DIR/<name>.npy, float64")
     return ap.parse_args()
 
 
@@ -65,11 +68,12 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def ncu_traffic(rows_local: int, d: int):
-    """dram bytes per K1 launch from the committed ncu capture, scaled to this launch's rows."""
+    """dram bytes per K1 launch from a stored ncu capture (profiles/k1_traffic.json), scaled to this launch's rows;
+    None when there is none for this d."""
     try:
         with open(os.path.join(ROOT, "profiles", "k1_traffic.json")) as f:
             t = json.load(f)
@@ -243,7 +247,7 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -312,6 +316,8 @@ def run_b200(args):
     barrier()
     t1 = time.time()
     clocks = sampler.stop(t0, t1) if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"weights": w, "loss_history": hist})
     dev_s = max_over_ranks(st.device_ms_total / 1e3)
     value = total_rows * st.passes / dev_s
     # the bit-identical memoised pass structure (AGD_FLAG_MEMOIZE_FX), reported beside the headline; like the headline it gets
@@ -352,11 +358,6 @@ def run_b200(args):
                 "frac_one_point": alg_bytes / (k1_ms_single * 1e-3) / 1e9 / peak,
                 "k1_share_of_step": st.k1_ms_total / st.device_ms_total}
 
-    # ---- e2e: public call with HOST buffers; shard upload + run + results inside the timed region
-    e2e = None
-    if not args.no_e2e:
-        e2e = measure_e2e(S, ctx, data, rows_local, total_rows, d, args, run, barrier, max_over_ranks, world)
-
     # ---- parity on the FULL workload (every N): the same loop on the GPU path and on the oracle, same rows
     parity = None
     if parity_iters > 0:
@@ -367,6 +368,12 @@ def run_b200(args):
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         res = cpu_reference(cpu_sample_rows(args), d, 2, 1)
         cpu = {k: res[k] for k in CPU_KEYS}
+
+    # ---- e2e: public call with HOST buffers; shard upload + run + results inside the timed region.  Last: its pinned host
+    # copy of the shard stays in torch's host cache, and parity / cpu_baseline hold host copies of their own
+    e2e = None
+    if not args.no_e2e:
+        e2e = measure_e2e(S, ctx, data, rows_local, total_rows, d, args, run, barrier, max_over_ranks, world)
 
     if rank == 0:
         wl_text = {"logistic_f32": f"logistic-loss AGD, {total_rows} x {d} dense {dict(f32='fp32', bf16='bf16 storage', f64='fp64 storage')[store]} "
@@ -414,6 +421,15 @@ def run_b200(args):
     data.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir: str, arrays: dict):
+    """What the timed run returned to its caller, one float64 .npy per array (d + the history length doubles: far
+    below 64 MB at any d the kernels take).  Inputs are seeded, so two builds given the same arguments can be compared
+    output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def measure_parity(S, data, run, iters, total_rows, rows_local, d, rank, world, barrier):

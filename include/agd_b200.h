@@ -1,17 +1,17 @@
 /*
- * agd_b200.h -- C-ABI of the B200-native accelerated-gradient-descent hot path.
+ * agd_b200.h -- C-ABI of the H100-native accelerated-gradient-descent hot path.
  *
  * This is the drop-in boundary a JVM binding (JNI) for staple/spark-agd would bind: plain
  * pointers and sizes, no C++/torch types.  Reference paths are relative to /root/reference:
  *   AGD.scala   = src/main/scala/org/apache/spark/mllib/optimization/AcceleratedGradientDescent.scala
  *   Suite.scala = src/test/scala/org/apache/spark/mllib/optimization/AcceleratedGradientDescentSuite.scala
  *
- * Model: one agd_handle per process owns one or more local B200s.  Each GPU pins one row-shard of
+ * Model: one agd_handle per process owns one or more local H100s.  Each GPU pins one row-shard of
  * the (n x d) design matrix in HBM (the analogue of `dataRDD.cache()`, Suite.scala:51).  A "pass" is
  * one applySmooth (AGD.scala:192-208): fused row-block gradient kernel over the shard, one
  * all-reduce of the packed [grad(d) | loss | count] fp64 buffer, and the fused O(d) update kernel.
  * All entry points return 0 on success, nonzero on error (see agd_last_error).  There is no CPU
- * fallback anywhere: without a usable sm_100 GPU every compute entry point fails.
+ * fallback anywhere: without a usable sm_90 GPU every compute entry point fails.
  *
  * Threading: agd_reserve / agd_load_* may be called concurrently for DIFFERENT local devices (Spark
  * task threads); everything else is single-caller, like the driver thread of AGD.scala:177.
@@ -95,7 +95,7 @@ int agd_abi_version(void);
 int agd_sizeof_params(void);
 int agd_sizeof_stats(void);
 void agd_default_params(agd_params *p);
-/* Opens n_dev local GPUs (device ordinals in device_ids).  Fails when a device is not sm_100. */
+/* Opens n_dev local GPUs (device ordinals in device_ids).  Fails when a device is not sm_90. */
 int agd_create(const int32_t *device_ids, int32_t n_dev, agd_handle **out);
 int agd_destroy(agd_handle *h);
 /* Message of the last failure on this handle (h may be NULL: last agd_create failure). */
@@ -182,13 +182,13 @@ int agd_smooth(agd_handle *h, int32_t gradient, const double *w, double *loss, d
 /* agd_smooth at w plus the loss (no gradient) at a second point w2, both from ONE sweep over the shards -- the fused form of
  * applySmooth(y) (AGD.scala:250) and the history evaluation applySmooth(x) (:304) that agd_run uses.  On dense shards every
  * output equals, bit for bit, what two agd_smooth calls return.  Fails on shards whose kernel has no two-point form
- * (tcgen05 bf16 path, d below one 16-row tile); agd_run then simply does not fuse. */
+ * (wgmma bf16 path, d below one 16-row tile); agd_run then simply does not fuse. */
 int agd_smooth_pair(agd_handle *h, int32_t gradient, const double *w, const double *w2, double *loss, double *grad,
                     int64_t *count, double *loss2);
 /* Two complete applySmooth evaluations (loss and gradient at w AND at w2) from ONE sweep over the shards -- what agd_run's
  * memoised pass structure uses to evaluate applySmooth(x) of the backtracking test (AGD.scala:269) together with
  * applySmooth(y) of the next iteration (:250).  Bit for bit what two agd_smooth calls return.  Dense fp32 / fp64 shards with
- * at most 512 16-byte vectors per row (d <= 2048 fp32, <= 1024 fp64) and bf16 shards on the tcgen05 kernel; fails elsewhere. */
+ * at most 512 16-byte vectors per row (d <= 2048 fp32, <= 1024 fp64) and bf16 shards on the wgmma kernel; fails elsewhere. */
 int agd_smooth_two(agd_handle *h, int32_t gradient, const double *w, const double *w2, double *loss, double *grad,
                    int64_t *count, double *loss2, double *grad2);
 /* agd_prox = applyProjector (AGD.scala:214-222): Updater.compute(w, g, step, iter = 1, reg). */

@@ -6,7 +6,7 @@ import org.apache.spark.mllib.linalg.{DenseVector, SparseVector, Vector, Vectors
 import org.apache.spark.rdd.RDD
 
 /** Drop-in for staple/spark-agd's optimizer: same package, class, constructor, setters, `optimize`
-  * and `run`, but the loop executes natively on the box's B200s through NativeAGD (JNI over
+  * and `run`, but the loop executes natively on the box's H100s through NativeAGD (JNI over
   * include/agd_b200.h).  Source only -- no JVM in the build image.
   *
   * Deployment: ONE executor JVM per GPU box (or `local[N]`), owning all of the box's GPUs.  Data path: each RDD
@@ -17,7 +17,7 @@ import org.apache.spark.rdd.RDD
   *   -Dagd.devices=0,1,...   GPUs of the box (default 0)
   *   -Dagd.store=f64|f32|bf16  HBM storage of dense features.  f64 (default) keeps every `Double` exact; f32 is the
   *                           benchmarked layout (half the bytes, twice the examples/s) and ROUNDS features to fp32 --
-  *                           exact when the RDD was built from floats; bf16 (d % 128 == 0) selects the tcgen05 kernel
+  *                           exact when the RDD was built from floats; bf16 (d % 128 == 0) selects the wgmma kernel
   *   -Dagd.flags=0|1|2       agd_params.flags: 0 = the reference's evaluations, fused sweeps; 1 = AGD_FLAG_MEMOIZE_FX;
   *                           2 = AGD_FLAG_NO_FUSE */
 @DeveloperApi

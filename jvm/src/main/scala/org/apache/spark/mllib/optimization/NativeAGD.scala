@@ -28,14 +28,14 @@ private[optimization] object NativeAGD {
     case _: LeastSquaresGradient => 1
     case _: HingeGradient => 2
     case other => throw new UnsupportedOperationException(
-      s"${other.getClass.getName} has no B200 kernel (Logistic/LeastSquares/Hinge only; there is no CPU fallback)")
+      s"${other.getClass.getName} has no H100 kernel (Logistic/LeastSquares/Hinge only; there is no CPU fallback)")
   }
   def updaterId(u: Updater): Int = u match {
     case _: SimpleUpdater => 0
     case _: SquaredL2Updater => 1
     case _: L1Updater => 2
     case other => throw new UnsupportedOperationException(
-      s"${other.getClass.getName} has no B200 kernel (Simple/SquaredL2/L1 only; there is no CPU fallback)")
+      s"${other.getClass.getName} has no H100 kernel (Simple/SquaredL2/L1 only; there is no CPU fallback)")
   }
 
   /** The one native handle of THIS JVM (an executor, or the driver in local mode): it owns the box's GPUs and keeps the

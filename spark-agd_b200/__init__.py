@@ -1,7 +1,7 @@
-"""spark-agd_b200: B200-native accelerated (proximal) gradient descent -- the hot path of
+"""spark-agd_b200: H100-native accelerated (proximal) gradient descent -- the hot path of
 staple/spark-agd (AcceleratedGradientDescent.optimize) behind the reference's own operator API.
 
-Layout: csrc/ holds the sm_100a CUDA kernels and the C-ABI (include/agd_b200.h); optimization.py is
+Layout: csrc/ holds the sm_90a CUDA kernels and the C-ABI (include/agd_b200.h); optimization.py is
 the host-side mirror of the reference interface.  The directory name carries a hyphen (the repo's
 naming contract); import it as `spark_agd_b200` through the loader module at the repo root.
 """

@@ -45,7 +45,7 @@ def _sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into spark-agd_b200/libagd_b200.so (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into spark-agd_b200/libagd_b200.so (nvcc cross-compiles
     without a GPU).  Rebuilds only when a source is newer than the library."""
     stale = (not os.path.exists(LIB_PATH)) or any(
         os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in _sources())
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose or res.returncode != 0:
             print(res.stdout)
         if res.returncode != 0:
-            raise RuntimeError("building libagd_b200.so failed (nvcc for sm_100a is required; there is no fallback)")
+            raise RuntimeError("building libagd_b200.so failed (nvcc for sm_90a is required; there is no fallback)")
     return LIB_PATH
 
 

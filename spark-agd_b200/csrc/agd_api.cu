@@ -1,6 +1,6 @@
 // agd_api.cu -- the C-ABI of include/agd_b200.h: handle, shard loading, the collective, and the
 // AcceleratedGradientDescent.run driver loop (AGD.scala:177-338) executed natively around the
-// K1 / all-reduce / K3 kernels.  No CPU fallback: every compute entry point needs an sm_100 GPU.
+// K1 / all-reduce / K3 kernels.  No CPU fallback: every compute entry point needs an sm_90 GPU.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <nccl.h>  // types and prototypes only; the library is dlopen'ed (torch ships its own libnccl.so.2)
@@ -122,11 +122,11 @@ struct agd_handle {
   bool comm_ready = false;
   bool comm_auto = false;   // the world is this process's own GPUs (agd_create): NCCL is only built if it is ever needed
   bool ipc_only = false;    // agd_comm_init_ipc: no NCCL at all, the host ships the CUDA IPC handles (agd_xchg_export/import)
-  int k1_variant = 0;  // 0 auto, 1 ring, 2 generic, 4 tcgen05 (bf16)
+  int k1_variant = 0;  // 0 auto, 1 ring, 2 generic, 4 wgmma (bf16)
   int ring_stages = 0;
   int tune_rows = 0, tune_ctas = 0, tune_full = 0;
   int k1_diag = 0;
-  int tc_margins_f64 = 0;    // tcgen05 kernel: fp64-exact margins instead of the fp32 phase 1
+  int tc_margins_f64 = 0;    // wgmma kernel: fp64-exact margins instead of the fp32 phase 1
   unsigned long long sample_seed = 0, sample_thresh = 0;  // mini-batch row mask of the current pass (0 = every row)
   int collective = 0;        // 0 = auto (peer memory if every pair of ranks can map each other, else NCCL), 1 = nccl, 2 = p2p
   int32_t x_d = 0;           // dimension the exchange buffers were built for (0 = not built)
@@ -236,7 +236,7 @@ int ensure_slabs(agd_handle *h, Dev &D, int blocks, int32_t n) {
 }
 
 // elem_bytes > 0: dense storage -- rows are padded with zero columns to whole 16-byte vectors when that puts the
-// shard on the TMA-ring / tcgen05 kernels.  The solver then runs in the padded dimension, which is bit-identical:
+// shard on the TMA-ring / wgmma kernels.  The solver then runs in the padded dimension, which is bit-identical:
 // the extra gradient entries are exactly 0, so the extra weights stay exactly 0 under every updater.
 int set_dim(agd_handle *h, int32_t d, int elem_bytes = 0) {
   std::lock_guard<std::mutex> g(h->mu);
@@ -530,7 +530,7 @@ void trace_report(agd_handle *h, const char *what) {
 
 typedef const double *(*WSel)(Dev &);
 
-// which K1 kernel a dense shard of this handle runs on (0 generic, 1 ring, 3 tcgen05)
+// which K1 kernel a dense shard of this handle runs on (0 generic, 1 ring, 3 wgmma)
 int dense_kernel_of(const agd_handle *h, int eb) {
   bool ring = k1_ring_supported(h->d, eb) != 0;
   if (h->k1_variant == 2) ring = false;
@@ -545,7 +545,7 @@ bool dual_supported(const agd_handle *h) {
     if (s.csr) continue;
     const int eb = s.elem_bytes ? s.elem_bytes : 4;
     const int k = dense_kernel_of(h, eb);
-    if (k == 3 && (h->tune_rows != 0 || h->tc_margins_f64)) return false;   // tcgen05: the default (fp32-margin) mapping has one
+    if (k == 3 && (h->tune_rows != 0 || h->tc_margins_f64)) return false;   // wgmma: the default (fp32-margin) mapping has one
     if (k == 1 && !k1_ring_dual_supported(h->d, eb)) return false;
   }
   return h->k1_diag == 0;
@@ -558,7 +558,7 @@ bool dual_full_supported(const agd_handle *h) {
     if (s.csr) return false;
     const int eb = s.elem_bytes ? s.elem_bytes : 4;
     const int k = dense_kernel_of(h, eb);
-    if (k == 3) { if (h->tune_rows != 0 || h->tc_margins_f64) return false; continue; }   // tcgen05: default mapping has one
+    if (k == 3) { if (h->tune_rows != 0 || h->tc_margins_f64) return false; continue; }   // wgmma: default mapping has one
     if (k != 1 || !k1_ring_dual_full_supported(h->d, eb)) return false;
   }
   return h->k1_diag == 0;
@@ -623,7 +623,7 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     bool ring = k1_ring_supported(d, eb) != 0;
     if (h->k1_variant == 2) ring = false;
     const bool tc = k1_tc_supported(d, eb) && (h->k1_variant == 0 || h->k1_variant == 4);
-    if (h->k1_variant == 4 && !tc) return fail(h, "tcgen05 kernel needs bf16 storage with d %% 128 == 0 and d <= 4096 (d=%d)", d);
+    if (h->k1_variant == 4 && !tc) return fail(h, "wgmma kernel needs bf16 storage with d %% 128 == 0 and d <= 4096 (d=%d)", d);
     if (h->k1_variant == 1 && !ring) return fail(h, "ring kernel does not support d=%d with %d-byte elements", d, eb);
     if (a.w2 && ((tc && (h->tune_rows != 0 || h->tc_margins_f64)) || (!tc && ring && !k1_ring_dual_supported(d, eb))))
       return fail(h, "internal: two-point sweep requested on a kernel without one");
@@ -825,8 +825,8 @@ int agd_create(const int32_t *device_ids, int32_t n_dev, agd_handle **out) {
     D.mu = new std::mutex();
     if (D.ordinal < 0 || D.ordinal >= count) { fail(h, "device ordinal %d out of range (0..%d)", D.ordinal, count - 1); agd_destroy(nh); return 1; }
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, D.ordinal) != cudaSuccess || prop.major != 10) {
-      fail(h, "device %d is not an sm_100 (Blackwell B200) GPU; kernels are built for sm_100a only", D.ordinal);
+    if (cudaGetDeviceProperties(&prop, D.ordinal) != cudaSuccess || prop.major != 9) {
+      fail(h, "device %d is not an sm_90 (Hopper H100) GPU; kernels are built for sm_90a only", D.ordinal);
       agd_destroy(nh);
       return 1;
     }
@@ -1260,7 +1260,7 @@ const char *agd_kernel_name(const agd_handle *h, int32_t dev) {
   const char *t = eb == 8 ? "double" : (eb == 4 ? "float" : "__nv_bfloat16");
   static thread_local char buf[96];
   switch (dense_kernel_of(h, eb)) {
-    case 3: return "k1_tc_kernel (tcgen05, bf16 storage)";
+    case 3: return "k1_tc_kernel (wgmma, bf16 storage)";
     case 1: snprintf(buf, sizeof buf, "k1_ring_kernel<%s,...>", t); return buf;
     default: snprintf(buf, sizeof buf, "k1_generic_kernel<%s>", t); return buf;
   }

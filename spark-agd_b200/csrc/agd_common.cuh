@@ -1,4 +1,4 @@
-// agd_common.cuh -- shared declarations of the sm_100a hot-path kernels (internal, not part of the ABI).
+// agd_common.cuh -- shared declarations of the sm_90a hot-path kernels (internal, not part of the ABI).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,7 +26,7 @@ struct K1Args {
   int32_t tune_rows;      // 0 = default; rows per tile of the headline ring shape (4|8)
   int32_t tune_ctas;      // 0 = default; resident CTAs per SM (1|2|3)
   int32_t tune_full;      // 0 = default; 1 = keep the column predicates even when every thread owns whole vectors
-  int32_t tc_margins_f64; // tcgen05 kernel: 1 = fp64-exact margins on the CUDA cores (option tc_margins=f64), 0 = fp32 (default)
+  int32_t tc_margins_f64; // wgmma kernel: 1 = fp64-exact margins on the CUDA cores (option tc_margins=f64), 0 = fp32 (default)
 };
 
 // launch helpers (k1_dense.cu); return the number of blocks that wrote a slab
@@ -37,7 +37,7 @@ int k1_ring_dual_full_supported(int32_t d, int elem_bytes);
 cudaError_t k1_generic_launch(const K1Args &a, int elem_bytes, int sm_count, int max_blocks, int *blocks_out,
                               cudaStream_t st);
 int k1_max_blocks(int sm_count);
-// bf16 shards: margins on CUDA cores, X^T r on tcgen05 (k1_tc.cu); d % 128 == 0, d <= 4096
+// bf16 shards: margins on CUDA cores, X^T r on wgmma (k1_tc.cu); d % 128 == 0, d <= 4096
 int k1_tc_supported(int32_t d, int elem_bytes);
 cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStream_t st);
 // ---------------------------------------------------------------- K2': one-shot all-reduce over NVLink peer memory

@@ -1,4 +1,4 @@
-// k1_csr.cu -- K1 for SparseVector rows stored as CSR (sm_100a).
+// k1_csr.cu -- K1 for SparseVector rows stored as CSR (sm_90a).
 //
 // Same contract as the dense kernel (seqOp fold of AGD.scala:197-200 with the sparse branches of
 // BLAS.dot / BLAS.axpy [mllib-1.3.0]): one warp per row, lanes stride the row's stored entries

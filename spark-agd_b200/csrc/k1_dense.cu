@@ -1,4 +1,4 @@
-// k1_dense.cu -- K1: fused row-block gradient kernel for dense shards (sm_100a).
+// k1_dense.cu -- K1: fused row-block gradient kernel for dense shards (sm_90a).
 //
 // One launch = the seqOp fold of applySmooth (AGD.scala:197-200) over one GPU's shard:
 //   m_i = x_i . w            (BLAS.dot inside Gradient.compute [mllib-1.3.0], call site AGD.scala:198)

@@ -1,21 +1,24 @@
-// k1_tc.cu -- K1 for bf16-stored dense shards: margins on the CUDA cores, X^T r on tcgen05 (sm_100a).
+// k1_tc.cu -- K1 for bf16-stored dense shards: margins on the CUDA cores, X^T r on wgmma (sm_90a).
 //
 // north_star's split for the bf16 configuration: the row tile is brought in ONCE by TMA tensor copies
 // (128B swizzle) and used twice without ever being widened into registers:
-//   phase 1 (CUDA cores, fp64): m_i = x_i . w  -- 256 consumer threads stream the 16-row tile out of
-//           shared memory, widen bf16 -> fp64 on the fly and FMA into 4 row accumulators per thread;
-//           nothing is retained, so the loop runs at streaming speed;
+//   phase 1 (CUDA cores): m_i = x_i . w  -- the consumer threads stream the 16-row tile out of shared
+//           memory, widen bf16 on the fly and FMA into row accumulators; nothing is retained, so the loop
+//           runs at streaming speed;
 //   scalar  (1 dedicated warp): margins -> loss', loss (k1_device.cuh); r_i = loss'_i is split into three
-//           bf16 pieces (hi / mid / lo, 24 mantissa bits) that form the B operand [N=16 x K=16 rows];
-//   phase 2 (tcgen05, fp32 in TMEM): D[c] (128 features x 16) += A (X^T chunk, MN-major view of the SAME
-//           swizzled tile) * B, one UTCHMMA per 128-feature chunk, issued by a single thread;
-//           every kFlush tiles the accumulators are read back (tcgen05.ld) and added into fp64 registers,
-//           so fp32 only ever holds sums over kFlush*16 rows.
-// Roles: warps 0-15 consumers, warp 16 TMA producer, warp 17 MMA issuer, warp 18 scalar, warps 20-23 own the fp64
-// gradient and flush TMEM; setmaxnreg moves registers from the consumers/aux warps to the flush warpgroup.  Shared-memory ring of 16 KB groups (8 blocks of [16 rows][64
-// features]); a group is released by the tcgen05.commit that follows the MMAs reading it.
-// Accuracy: margins and losses are fp64-exact like the other kernels; the gradient carries the bf16x3
-// split (2^-24) and fp32 partial sums, i.e. ~1e-7 relative (tests/test_gpu_parity.py states the bound).
+//           bf16 pieces (hi / mid / lo, 24 mantissa bits) that form the B operand [K=16 rows x N columns];
+//   phase 2 (wgmma, fp32 in registers): D (64 features x N) = A (X^T block, MN-major view of the SAME swizzled
+//           tile) * B, two wgmma.m64nNk16 per 128 features, issued by one warpgroup; each result (a sum over
+//           the tile's 16 rows) is added into fp64 registers right away.
+// The pieces are replicated across B's columns so that every lane of the accumulator fragment holds hi, mid
+// and lo of its own two features (column 2j: hi, 2j+1: mid, 8+2j: lo for lane j of a quad): no shuffles.
+// Roles: warps 0-15 consumers, warp 16 TMA producer, warp 18 scalar, warps 20-23 the MMA warpgroup that owns
+// the fp64 gradient; setmaxnreg moves registers from the consumers/aux warps to the MMA warpgroup.  Shared-memory
+// ring of groups of gb blocks of [16 rows][64 features] (gb = the largest even divisor of d / 64 that is <= 8, so a tile is
+// a whole number of groups for every role); a group is released once the wgmmas reading it
+// have completed in all four MMA warps.
+// Accuracy: the gradient carries the bf16x3 split (2^-24) and fp32 sums over 16 rows, i.e. ~1e-7 relative
+// (tests/test_gpu_parity.py states the bound).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -29,13 +32,13 @@ namespace agd {
 namespace {
 
 constexpr int kKR = 16;            // rows per tile = K of one MMA
-// RPT = rows per consumer thread.  RPT = 2: 512 consumers (+ 256 aux/flush threads, setmaxnreg 64/56/112 out of the 80 at
+// RPT = rows per consumer thread.  RPT = 2: 512 consumers (+ 256 aux/MMA threads, setmaxnreg 64/56/168 out of the 80 at
 // launch).  RPT = 4: 256 consumers, each w value fetched from shared memory serves four rows instead of two -- the kernel is
 // bound by shared-memory bandwidth (TMA writes + MMA operand reads + x reads + w reads), and w is the largest reader.
-constexpr int kRegsConsumer = 64, kRegsAux = 56, kRegsFlush = 112;
-constexpr int kRegsFlush2 = 168;   // two-gradient form: 80 + everything released by 512 consumers (16 each) and 128 aux threads (24 each)
-constexpr int kFlush = 8;          // tiles between TMEM -> fp64 flushes (128 rows of fp32 accumulation)
+// MMA warpgroup: 80 at launch + everything released by 512 consumers (16 each) and 128 aux threads (24 each)
+constexpr int kRegsConsumer = 64, kRegsAux = 56, kRegsMma = 168;
 constexpr int kBlockBytes = kKR * 128;     // one [16 rows][64 features] swizzled block
+constexpr int kBBytes = 1024;              // one B operand buffer: [N <= 24 columns][16 rows] bf16, K-major, no swizzle
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -79,22 +82,68 @@ __device__ __forceinline__ void tma_tile_3d(uint32_t dst, const CUtensorMap *map
                "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// sm_90 shared-memory matrix descriptor: start, leading / stride byte offsets (16-byte units), layout type in bits 62-63
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo, uint32_t sbo, uint64_t layout) {
+  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | (layout << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] = A[64 x 16] * B[16 x N], bf16 in, fp32 out (scale-d = 0: nothing is accumulated); A MN-major (transposed)
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc);
+template <>
+__device__ __forceinline__ void wgmma_bf16<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, 0, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 1, 0; }"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(adesc), "l"(bdesc)
+               : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<24>(float (&d)[12], uint64_t adesc, uint64_t bdesc) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, 0, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 1, 0; }"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+               : "l"(adesc), "l"(bdesc)
+               : "memory");
+}
+
+// MMA warpgroup: adds the owned feature's hi + mid + lo (and hi2 + mid2 + lo2) of a 128-feature pair into fp64.  Fragment
+// index for row-half 0 (row-half 1: + 2): hi 0, mid 1, lo 4, hi2 5, mid2 8, lo2 9.
+template <int N, bool TWO>
+__device__ __forceinline__ void mma_accumulate(const float (&e)[2][N / 2], int hb, int hs, double &g, double *g2) {
+  float v[6];
+#pragma unroll
+  for (int t = 0; t < (TWO ? 6 : 3); ++t) {
+    const int i = t == 0 ? 0 : t == 1 ? 1 : t == 2 ? 4 : t == 3 ? 5 : t == 4 ? 8 : 9;
+    const float x0 = hs ? e[0][i + 2] : e[0][i], x1 = hs ? e[1][i + 2] : e[1][i];
+    v[t] = hb ? x1 : x0;
+  }
+  g += ((double)v[0] + (double)v[1]) + (double)v[2];
+  if (TWO) *g2 += ((double)v[3] + (double)v[4]) + (double)v[5];
+}
+// the ring group may be refilled once all four MMA warps are done with it
+__device__ __forceinline__ void mma_release(uint32_t empty_bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(empty_bar);
 }
 
 struct TcLayout {
-  uint32_t ring_off, w_off, b2_off, partial_off, bars_off, tmem_off, total;
+  uint32_t ring_off, w_off, b2_off, partial_off, bars_off, g2_off, total;
 };
-__host__ __device__ inline TcLayout tc_layout(int ring_groups, int group_bytes, int d) {
+// g2: the fp64 gradient at the second point of the two-gradient form (one owner thread per entry)
+__host__ __device__ inline TcLayout tc_layout(int ring_groups, int group_bytes, int d, bool two_gradient) {
   TcLayout L;
   L.ring_off = 0;
   L.w_off = (uint32_t)ring_groups * group_bytes;
   L.b2_off = L.w_off + (uint32_t)d * 8;
-  L.partial_off = L.b2_off + 2 * 512;
+  L.partial_off = L.b2_off + 2 * kBBytes;
   L.bars_off = L.partial_off + 2 * kKR * 16 * 8;
-  L.tmem_off = L.bars_off + (2 * (uint32_t)ring_groups + 8) * 8;
-  L.total = L.tmem_off + 16;
+  L.g2_off = L.bars_off + (2 * (uint32_t)ring_groups + 8) * 8;
+  L.total = L.g2_off + (two_gradient ? (uint32_t)d * 8 : 0u);
   return L;
 }
 
@@ -107,10 +156,9 @@ struct TcArgs {
   int d, kind, slab_stride;
   unsigned long long sample_seed, sample_thresh;
   long long row_base;
-  int gb;           // 64-feature blocks per ring group (<= 8)
+  int gb;           // 64-feature blocks per ring group: the largest even divisor of d / 64 that is <= 8
   int ngt;          // groups per tile = d / (64 * gb)
   int ring_groups;  // ring capacity in groups
-  int tmem_cols;    // power of two >= max(32, d / 8)
   int one_copy;     // 1: a ring group arrives as ONE 3-D TMA copy [gb blocks][16 rows][64 features] instead of gb 2-D copies
   int diag;         // option k1_diag: 100 = consumers skip the arithmetic, 101 = the MMAs are not issued (timing bisection only)
 };
@@ -118,11 +166,12 @@ struct TcArgs {
 // RPT = 0 selects the row-per-lane consumer mapping: a warp covers all 16 rows of the tile for two adjacent 8-feature chunks,
 // so its w reads are broadcasts (one shared-memory wavefront instead of four) and each lane owns one row's partial dot.
 __host__ __device__ constexpr int tc_consumers(int rpt) { return rpt == 4 ? 256 : 512; }
-// packed fp32 FMA (SASS FFMA2): d.{x,y} = a.{x,y} * b.{x,y} + c.{x,y}
+// fp32 FMA on a packed pair: d.{x,y} = a.{x,y} * b.{x,y} + c.{x,y}, two round-to-nearest FMAs
 __device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  const float x = __fmaf_rn(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)c));
+  const float y = __fmaf_rn(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)),
+                            __uint_as_float((uint32_t)(c >> 32)));
+  return ((unsigned long long)__float_as_uint(y) << 32) | __float_as_uint(x);
 }
 __device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
   unsigned long long d;
@@ -131,62 +180,52 @@ __device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
 }
 
 // F32: phase 1 in fp32 (option tc_margins=f32, the default): a bf16 is the upper half of an fp32, so widening is one ALU op
-// and there is no fp64 conversion per element; products are accumulated by packed fp32 FMAs over at most 8 terms per
+// and there is no fp64 conversion per element; products are accumulated by fp32 FMAs on packed pairs over at most 8 terms per
 // accumulator and then added into the fp64 row sums.  Margins carry ~2^-23 relative to sum |x_i w_i| (w rounded to fp32) --
-// the same class as the gradient of this kernel (bf16 x 3 split, fp32 TMEM sums).  F32 = false keeps fp64-exact margins.
+// the same class as the gradient of this kernel (bf16 x 3 split, fp32 tensor-core sums).  F32 = false keeps fp64-exact margins.
 // DUAL (F32 mapping only): the loss is also evaluated at a second point w2 from the same tile -- one more packed FMA per
 // feature pair in phase 1, lanes 16-31 of the scalar warp -- with bits identical to a launch of its own at w2.
-// DUAL == 2: the GRADIENT at w2 as well (two-gradient sweep): r at w2 takes columns 3-5 of the same B operand, so the second
-// X^T r costs no extra MMA at all -- the tensor core computes 16 columns either way; the flush reads 8 TMEM columns
-// instead of 4 and keeps a second fp64 gradient (setmaxnreg gives the flush warpgroup everything the others released).
+// DUAL == 2: the GRADIENT at w2 as well (two-gradient sweep): r at w2 takes columns 2j+9, 16+2j and 17+2j of a 24-column B
+// operand (hi2, mid2, lo2 for lane j of a quad), so the second X^T r costs no extra MMA instruction; its fp64 gradient
+// lives in shared memory (g2), each entry owned by the one MMA thread that updates it.
 template <int RPT, bool F32, int DUAL = 0>
 __global__ void __launch_bounds__(tc_consumers(RPT) + 256, 1)
 k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap3, const TcArgs a,
              const long long ntiles) {
   constexpr int kConsumers = tc_consumers(RPT);   // RPT > 0: 64 threads (one 16-byte vector each) per group row
-  constexpr int kThreads = kConsumers + 256;   // + warpgroup (producer, MMA issuer, scalar, idle) + flush warpgroup
+  constexpr int kThreads = kConsumers + 256;   // + warpgroup (producer, idle, scalar, idle) + MMA warpgroup
+  constexpr int kN = DUAL == 2 ? 24 : 16;      // B columns: (hi, mid) x 4, (lo, hi2) x 4 [, (mid2, lo2) x 4]
   constexpr int kCW = kConsumers / 32;         // consumer warps; the aux warps follow
   constexpr bool kRepartition = RPT != 4;      // 768 threads start with 80 registers: move some to the flush warpgroup
   extern __shared__ __align__(1024) unsigned char smem[];
   const int group_bytes = a.gb * kBlockBytes;
-  const TcLayout L = tc_layout(a.ring_groups, group_bytes, a.d);
+  const TcLayout L = tc_layout(a.ring_groups, group_bytes, a.d, DUAL == 2);
   double *w_s = reinterpret_cast<double *>(smem + L.w_off);
-  unsigned char *b2 = smem + L.b2_off;                                       // [2][512 B]
+  unsigned char *b2 = smem + L.b2_off;                                       // [2][kBBytes]
   double *partial = reinterpret_cast<double *>(smem + L.partial_off);         // [2][16 rows][2] (RPT > 0) or [2][16 rows][16 warps]
   const uint32_t bars = smem_u32(smem + L.bars_off);
   const int RG = a.ring_groups;
-  // full[g] = bars + 8g ; empty[g] = bars + 8(RG+g) ; then wbar, b2_full[2], b2_empty[2], tile_done, flush_done
-  const uint32_t wbar = bars + 16u * RG, b2_full = wbar + 8, b2_empty = b2_full + 16, tile_done = b2_empty + 16,
-                 flush_done = tile_done + 8;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + L.tmem_off);
+  // full[g] = bars + 8g ; empty[g] = bars + 8(RG+g) ; then wbar, b2_full[2], b2_empty[2]
+  const uint32_t wbar = bars + 16u * RG, b2_full = wbar + 8, b2_empty = b2_full + 16;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long my_tiles = (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
-  const int nch = a.d / 128;
+  const int npairs = a.d / 128;   // 128-feature pairs of 64-feature blocks
   double *slab = a.slabs + (size_t)blockIdx.x * a.slab_stride;
 
   if (tid == 0) {
     for (int g = 0; g < RG; ++g) {
       mbar_init(bars + 8u * g, 1);
-      mbar_init(bars + 8u * (RG + g), 1);
+      mbar_init(bars + 8u * (RG + g), 4);   // one arrival per MMA warp
     }
     mbar_init(wbar, 1);
     mbar_init(b2_full, 1); mbar_init(b2_full + 8, 1);
-    mbar_init(b2_empty, 1); mbar_init(b2_empty + 8, 1);
-    mbar_init(tile_done, 1);
-    mbar_init(flush_done, 4);
+    mbar_init(b2_empty, 4); mbar_init(b2_empty + 8, 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(a.tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  // B operand rows 3..15 (unused N columns) stay zero for the whole kernel
-  for (int i = tid; i < 2 * 512 / 4; i += kThreads) reinterpret_cast<uint32_t *>(b2)[i] = 0u;
+  // B operand columns nobody writes (2j+9 without a second gradient) stay zero for the whole kernel
+  for (int i = tid; i < 2 * kBBytes / 4; i += kThreads) reinterpret_cast<uint32_t *>(b2)[i] = 0u;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp >= kCW && warp < kCW + 4) {
    if (kRepartition) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsAux));
@@ -212,40 +251,6 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
               tma_tile_2d(smem_u32(smem + (size_t)slot * group_bytes + b * kBlockBytes), &tmap, (gi * a.gb + b) * 64, (int)row0, full);
           }
         }
-      }
-    }
-   } else if (warp == kCW + 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      // instr desc: D=F32, A=B=BF16, A MN-major, B K-major, N=16, M=128
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
-      int slot = -1;
-      uint32_t flush_parity = 0;
-      for (long long k = 0; k < my_tiles; ++k) {
-        const int bb = (int)(k & 1);
-        mbar_wait(b2_full + 8u * bb, (uint32_t)((k >> 1) & 1));
-        const bool fresh = (k % kFlush) == 0;  // accumulators were just flushed (or never written)
-        if (fresh && k > 0) { mbar_wait(flush_done, flush_parity); flush_parity ^= 1u; }
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        const uint64_t bdesc = (uint64_t)((smem_u32(b2 + bb * 512) & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) |
-                               ((uint64_t)(256 >> 4) << 32) | (1ull << 46);
-        for (int gi = 0; gi < a.ngt; ++gi) {
-          if (++slot == RG) slot = 0;
-          for (int cc = 0; cc < a.gb / 2; ++cc) {
-            const uint32_t a_addr = smem_u32(smem + (size_t)slot * group_bytes + (2 * cc) * kBlockBytes);
-            const uint64_t adesc = (uint64_t)((a_addr & 0x3FFFF) >> 4) | ((uint64_t)(kBlockBytes >> 4) << 16) |
-                                   ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-            const uint32_t taddr = tmem_base + (uint32_t)(gi * (a.gb / 2) + cc) * 16u;
-            const uint32_t acc = fresh ? 0u : 1u;
-            if (a.diag != 101)
-            asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p; }" ::"r"(taddr),
-                         "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-                         : "memory");
-          }
-          umma_commit(bars + 8u * (RG + slot));  // the group may be refilled once these MMAs have read it
-        }
-        umma_commit(b2_empty + 8u * bb);
-        if (((k + 1) % kFlush) == 0 || k + 1 == my_tiles) umma_commit(tile_done);
       }
     }
    } else if (warp == kCW + 2) {
@@ -291,16 +296,23 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
       named_arrive(3 + bb, kConsumers + 32);                   // partial[bb] may be overwritten
       if (k >= 2) mbar_wait(b2_empty + 8u * bb, (uint32_t)(((k >> 1) - 1) & 1));  // MMAs of tile k-2 have read b2[bb]
       if (lane < kKR || (DUAL == 2 && second)) {
-        // r_i -> three bf16 pieces; element (n, row) of the K-major B operand (n = 0..2 at w, 3..5 at w2)
+        // r_i -> three bf16 pieces, each written to four columns of the K-major B operand: element (n, row) sits at
+        // (n / 8) * 256 + (row / 8) * 128 + (n % 8) * 16 + (row % 8) * 2.  At w: hi -> 2t, mid -> 2t+1, lo -> 8+2t;
+        // at w2: hi2 -> 9+2t, mid2 -> 16+2t, lo2 -> 17+2t (t = 0..3)
         const __nv_bfloat16 hi = __double2bfloat16(mult);
         const double r1 = mult - (double)__bfloat162float(hi);
         const __nv_bfloat16 mid = __double2bfloat16(r1);
         const double r2 = r1 - (double)__bfloat162float(mid);
         const __nv_bfloat16 lo = __double2bfloat16(r2);
-        unsigned char *base = b2 + bb * 512 + (srow / 8) * 128 + (srow % 8) * 2 + (second ? 3 * 16 : 0);
-        *reinterpret_cast<__nv_bfloat16 *>(base + 0 * 16) = hi;
-        *reinterpret_cast<__nv_bfloat16 *>(base + 1 * 16) = mid;
-        *reinterpret_cast<__nv_bfloat16 *>(base + 2 * 16) = lo;
+        const int n0 = second ? 9 : 0, n1 = second ? 16 : 1, n2 = second ? 17 : 8;
+        unsigned char *base = b2 + bb * kBBytes + (srow / 8) * 128 + (srow % 8) * 2;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const int c0 = n0 + 2 * t, c1 = n1 + 2 * t, c2 = n2 + 2 * t;
+          *reinterpret_cast<__nv_bfloat16 *>(base + (c0 / 8) * 256 + (c0 % 8) * 16) = hi;
+          *reinterpret_cast<__nv_bfloat16 *>(base + (c1 / 8) * 256 + (c1 % 8) * 16) = mid;
+          *reinterpret_cast<__nv_bfloat16 *>(base + (c2 / 8) * 256 + (c2 % 8) * 16) = lo;
+        }
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
@@ -322,54 +334,58 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
     }
    }
   } else if (warp >= kCW + 4) {
-    // ===================== flush warpgroup: owns the fp64 gradient(s), drains TMEM every kFlush tiles ==========
-    if (kRepartition) {
-      if (DUAL == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsFlush2));
-      else asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsFlush));
-    }
-    const int fw = warp - (kCW + 4);   // TMEM lanes 32*fw .. 32*fw+31 (kCW + 4 is a multiple of 4)
-    double gacc[32];                // feature (c*128 + 32*fw + lane), c < d/128
-    double gacc2[DUAL == 2 ? 32 : 1];   // the same at w2
+    // ===================== MMA warpgroup: X^T r on wgmma, owns the fp64 gradient(s) =====================
+    if (kRepartition) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsMma));
+    const int mw = warp - (kCW + 4);   // warp of the warpgroup (kCW + 4 is a multiple of 4)
+    const int q = lane >> 2, j = lane & 3;
+    // accumulator fragment of wgmma.m64nNk16: lane (q, j) of warp mw holds rows 16 mw + q and 16 mw + q + 8 (features of the
+    // 64-feature block), columns {2j, 2j+1} + 8i.  Within a 128-feature pair, this thread owns block (j >> 1), row-half (j & 1).
+    const int hb = j >> 1, hs = j & 1;
+    const int fo = 64 * hb + 16 * mw + q + 8 * hs;
+    double gacc[32];                // feature 128 p + fo, p < d / 128
 #pragma unroll
-    for (int c = 0; c < 32; ++c) { gacc[c] = 0.0; if (DUAL == 2) gacc2[DUAL == 2 ? c : 0] = 0.0; }
-    uint32_t done_parity = 0;
+    for (int p = 0; p < 32; ++p) gacc[p] = 0.0;
+    double *g2 = reinterpret_cast<double *>(smem + L.g2_off);   // DUAL == 2: the gradient at w2
+    if (DUAL == 2)
+      for (int p = 0; p < npairs; ++p) g2[128 * p + fo] = 0.0;
+    const int hp = a.gb / 2;        // pairs per ring group
+    int slot = -1;
+    uint32_t par = 1;
+    float acc[2][kN / 2];           // [block of the pair][fragment]
     for (long long k = 0; k < my_tiles; ++k) {
-      if (((k + 1) % kFlush) == 0 || k + 1 == my_tiles) {
-        mbar_wait(tile_done, done_parity);
-        done_parity ^= 1u;
-        asm volatile("tcgen05.fence::after_thread_sync;");
+      const int bb = (int)(k & 1);
+      mbar_wait(b2_full + 8u * bb, (uint32_t)((k >> 1) & 1));
+      const uint64_t bdesc = gmma_desc(smem_u32(b2 + bb * kBBytes), 128, 256, 0);   // K-major, no swizzle
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          if (c < nch) {
-            const uint32_t taddr = tmem_base + ((uint32_t)(fw * 32) << 16) + (uint32_t)c * 16u;
-            if (DUAL == 2) {
-              uint32_t v0, v1, v2, v3, v4, v5, v6, v7;
-              asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                           : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3), "=r"(v4), "=r"(v5), "=r"(v6), "=r"(v7)
-                           : "r"(taddr));
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-              gacc[c] += ((double)__uint_as_float(v0) + (double)__uint_as_float(v1)) + (double)__uint_as_float(v2);
-              gacc2[DUAL == 2 ? c : 0] += ((double)__uint_as_float(v3) + (double)__uint_as_float(v4)) + (double)__uint_as_float(v5);
-            } else {
-              uint32_t v0, v1, v2, v3;
-              asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                           : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3)
-                           : "r"(taddr));
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-              gacc[c] += ((double)__uint_as_float(v0) + (double)__uint_as_float(v1)) + (double)__uint_as_float(v2);
-            }
+      for (int p = 0; p < 32; ++p) {
+        if (p < npairs) {
+          const int pg = p % hp;
+          if (pg == 0) {
+            if (++slot == RG) slot = 0;
+            if (slot == 0) par ^= 1u;
+            mbar_wait(bars + 8u * slot, par);
           }
+          const uint32_t a0 = smem_u32(smem + (size_t)slot * group_bytes + (2 * pg) * kBlockBytes);
+          wgmma_fence();
+          if (a.diag != 101) {
+            // A: [64 features][16 rows] MN-major, 128B swizzle, 8-row groups 1024 B apart
+            wgmma_bf16<kN>(acc[0], gmma_desc(a0, kBlockBytes, 1024, 1), bdesc);
+            wgmma_bf16<kN>(acc[1], gmma_desc(a0 + kBlockBytes, kBlockBytes, 1024, 1), bdesc);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          mma_accumulate<kN, DUAL == 2>(acc, hb, hs, gacc[p], g2 + 128 * p + fo);
+          if (pg == hp - 1) mma_release(bars + 8u * (RG + slot), lane);   // last pair of the group
         }
-        asm volatile("tcgen05.fence::before_thread_sync;");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(flush_done);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(b2_empty + 8u * bb);   // B[bb] may be rewritten (tile k + 2)
     }
 #pragma unroll
-    for (int c = 0; c < 32; ++c)
-      if (c < nch) {
-        slab[c * 128 + fw * 32 + lane] = gacc[c];
-        if (DUAL == 2) slab[a.d + 4 + c * 128 + fw * 32 + lane] = gacc2[DUAL == 2 ? c : 0];
+    for (int p = 0; p < 32; ++p)
+      if (p < npairs) {
+        slab[128 * p + fo] = gacc[p];
+        if (DUAL == 2) slab[a.d + 4 + 128 * p + fo] = g2[128 * p + fo];
       }
   } else {
     // ===================== consumers: phase 1 in fp64, straight out of the swizzled tile =====================
@@ -592,12 +608,6 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
     }  // fp64 margins
     }  // column-slice mapping
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(a.tmem_cols));
-  }
 }
 
 // the opt-in shared-memory size is a per-device property of a function: set it when it changes, not on every launch
@@ -642,12 +652,16 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return cudaErrorInvalidValue;
+  // a tile is a whole number of ring groups, and a group a whole number of 128-feature pairs (d / 64 is even): every role
+  // (TMA producer, consumers, MMA warpgroup) then walks the same groups
+  const int nblk = a.d / 64;
+  int gb = 8;
+  while (nblk % gb) gb -= 2;
   CUtensorMap tmap3;
   {
-    const cuuint64_t gdim3[3] = {64, (cuuint64_t)a.rows, (cuuint64_t)(a.d / 64)};
+    const cuuint64_t gdim3[3] = {64, (cuuint64_t)a.rows, (cuuint64_t)nblk};
     const cuuint64_t gstr3[2] = {(cuuint64_t)a.d * 2, 128};
-    const int nblk3 = a.d / 64;
-    const cuuint32_t box3[3] = {64, (cuuint32_t)kKR, (cuuint32_t)(nblk3 < 8 ? nblk3 : 8)};
+    const cuuint32_t box3[3] = {64, (cuuint32_t)kKR, (cuuint32_t)gb};
     const cuuint32_t estr3[3] = {1, 1, 1};
     if (encode(&tmap3, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(a.X), gdim3, gstr3, box3, estr3,
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -661,19 +675,17 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
   t.labels = a.labels; t.w = a.w; t.w2 = a.w2; t.slabs = a.slabs; t.rows = a.rows; t.d = a.d; t.kind = a.kind;
   t.slab_stride = a.slab_stride;
   t.sample_seed = a.sample_seed; t.sample_thresh = a.sample_thresh; t.row_base = a.row_base;
-  const int nblk = a.d / 64;
-  t.gb = nblk < 8 ? nblk : 8;
-  t.ngt = nblk / t.gb;
+  t.gb = gb;
+  t.ngt = nblk / gb;
   const int group_bytes = t.gb * kBlockBytes;
   int ring = a.stages > 0 ? a.stages : 16;
-  const uint32_t budget = 227u * 1024u - 2048u;
-  while (ring > 2 && tc_layout(ring, group_bytes, a.d).total + 1024 > budget) --ring;
+  const bool two_gradient = a.w2 && a.dual_full;
+  const uint32_t budget = 227u * 1024u - 2048u;   // H100: 227 KB of shared memory per block
+  while (ring > 2 && tc_layout(ring, group_bytes, a.d, two_gradient).total + 1024 > budget) --ring;
   if (ring < t.ngt + 1) ring = t.ngt + 1;  // at least one tile and a bit
   t.ring_groups = ring;
-  int cols = 32;
-  while (cols < a.d / 8) cols <<= 1;
-  t.tmem_cols = cols;
-  const TcLayout L = tc_layout(ring, group_bytes, a.d);
+  const TcLayout L = tc_layout(ring, group_bytes, a.d, two_gradient);
+  if (L.total + 1024 > budget) return cudaErrorInvalidValue;
   const long long ntiles = (a.rows + kKR - 1) / kKR;
   long long grid = sm_count;
   if (grid > ntiles) grid = ntiles;
@@ -700,7 +712,7 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
     e = set_smem_once<4>(k1_tc_kernel<2, true, 1>, smem_bytes);
     if (e != cudaSuccess) return e;
     k1_tc_kernel<2, true, 1><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else {  // default: the same mapping with fp32 phase-1 arithmetic (packed FFMA2, no fp64 conversion per element)
+  } else {  // default: the same mapping with fp32 phase-1 arithmetic (fp32 FMAs on packed pairs, no fp64 conversion per element)
     e = set_smem_once<5>(k1_tc_kernel<2, true, 0>, smem_bytes);
     if (e != cudaSuccess) return e;
     k1_tc_kernel<2, true, 0><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);

@@ -1,4 +1,4 @@
-// k3_update.cu -- K3: fused O(d) vector kernels of the driver loop (sm_100a).
+// k3_update.cu -- K3: fused O(d) vector kernels of the driver loop (sm_90a).
 //
 // Replaces, on the device and in one launch per applySmooth result:
 //   grad / count                                  AGD.scala:207

@@ -191,7 +191,7 @@ __global__ void csr_validate_kernel(const long long *rowptr, long long rows, con
 
 inline unsigned grid_for(long long total) {
   long long g = (total + 255) / 256;
-  if (g > 148LL * 16) g = 148LL * 16;
+  if (g > 132LL * 16) g = 132LL * 16;   // 16 CTAs per H100 SM
   if (g < 1) g = 1;
   return (unsigned)g;
 }

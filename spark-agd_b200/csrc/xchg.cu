@@ -130,14 +130,14 @@ __global__ void __launch_bounds__(256) xchg_rs_gather_kernel(const double *xbuf,
 
 cudaError_t xchg_rs_publish_launch(const double *acc, const XchgRs &x, cudaStream_t st) {
   int grid = (x.n + 255) / 256;
-  if (grid > 296) grid = 296;
+  if (grid > 264) grid = 264;
   xchg_rs_publish_kernel<<<grid, 256, 0, st>>>(acc, x);
   return cudaGetLastError();
 }
 cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st) {
   const int l = (x.n + x.world - 1) / x.world;
   int grid = (l + 255) / 256;
-  if (grid > 148) grid = 148;
+  if (grid > 132) grid = 132;   // one CTA per H100 SM
   if (grid < 1) grid = 1;
   xchg_rs_reduce_bcast_kernel<<<grid, 256, 0, st>>>(xbuf_local, flags_local, x);
   return cudaGetLastError();
@@ -145,7 +145,7 @@ cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned
 cudaError_t xchg_rs_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
                                   int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st) {
   int grid = (n + 255) / 256;
-  if (grid > 296) grid = 296;
+  if (grid > 264) grid = 264;
   xchg_rs_gather_kernel<<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
   return cudaGetLastError();
 }

@@ -1,5 +1,5 @@
 """bench.py prints ONE JSON line with the keys the driver reads (task contract): the reference arm on the CPU here, the
-B200 arm on a GPU box with a small shard."""
+GPU arm on an H100 with a small shard."""
 import json
 import os
 import subprocess

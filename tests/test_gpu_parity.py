@@ -189,23 +189,22 @@ def tc_shape(d):
 @pytest.mark.parametrize("variant", ["auto", "auto-f64", "ring"])
 @pytest.mark.parametrize("grad", ["logistic", "least_squares", "hinge"])
 @pytest.mark.parametrize("shape", [(3001, 1024), (2000, 512), (515, 256), (777, 2048), (300, 4096), (129, 1104),
-                                   (37, 40), (10, 20000), (64, 8192), (5, 3), (4099, 128), (33, 3072)])
+                                   (37, 40), (10, 20000), (64, 8192), (5, 3), (4099, 128), (33, 3072), (517, 768),
+                                   (260, 640)])
 def test_bf16_storage_matches_oracle(agd, ctx, oracle, grad, shape, variant):
     """X stored as bf16 in HBM (rounded to nearest-even at load).  `ring`/generic: fp64 CUDA-core path, same
-    tolerances as fp32 storage.  `auto` on d % 128 == 0, d <= 4096 is the tcgen05 kernel: X^T r on the tensor cores with r
-    split into three bf16 pieces and fp32 partial sums over 128 rows -> gradient to 2e-6; margins on the CUDA cores, by
+    tolerances as fp32 storage.  `auto` on d % 128 == 0, d <= 4096 is the wgmma kernel: X^T r on the tensor cores with r
+    split into three bf16 pieces and fp32 partial sums over 16 rows -> gradient to 2e-6; margins on the CUDA cores, by
     default in fp32 (w rounded to fp32, packed FMAs over at most 8 terms, then fp64) -> loss to 2e-6, or fp64-exact with
-    option tc_margins=f64 (`auto-f64`) -> loss to 1e-12."""
+    option tc_margins=f64 (`auto-f64`) -> loss to 1e-12.  Off the tensor path `auto-f64` checks that the option changes
+    nothing, and `ring` forces the generic CUDA-core kernel (auto takes the ring wherever the ring fits)."""
     n, d = shape
     rng = np.random.default_rng(3000 + n + d)
     X, y = make_data(rng, n, d, grad, np.float32)
     w = rng.standard_normal(d) * 0.3 / np.sqrt(d) * 4
     ds = ctx.parallelize(y, X, store="bf16")
-    if variant != "auto" and not tc_shape(d):
-        ds.close()
-        pytest.skip("same kernel as auto")
     if variant == "ring":
-        ds.set_option("k1_variant", "ring")
+        ds.set_option("k1_variant", "ring" if tc_shape(d) else "generic")
     if variant == "auto-f64":
         ds.set_option("tc_margins", "f64")
     raw, yb = ds.get_rows(0, 0, n, dtype=np.uint16)
@@ -224,9 +223,9 @@ def test_bf16_storage_matches_oracle(agd, ctx, oracle, grad, shape, variant):
 
 @pytest.mark.parametrize("rows_opt,copy_opt", [(0, 0), (0, 2), (1, 0), (1, 2), (4, 0), (4, 2)])
 @pytest.mark.parametrize("shape,grad", [((3001, 1024), "logistic"), ((300, 4096), "least_squares"), ((515, 256), "hinge"),
-                                        ((1000, 128), "logistic"), ((130, 3072), "least_squares")])
+                                        ((1000, 128), "logistic"), ((130, 3072), "least_squares"), ((517, 768), "hinge")])
 def test_tc_kernel_forms(agd, ctx, oracle, shape, grad, rows_opt, copy_opt):
-    """The tcgen05 kernel's consumer mappings (ring_rows: 0 = default, two rows per thread of the column-slice mapping; 4 = four
+    """The wgmma kernel's consumer mappings (ring_rows: 0 = default, two rows per thread of the column-slice mapping; 4 = four
     rows per thread; 1 = row per lane with broadcast w reads) and its two TMA forms (default: one 3-D copy per ring group;
     ring_ctas=2: one 2-D copy per 64-feature block) all meet the tolerances of the tensor path."""
     n, d = shape
@@ -468,7 +467,7 @@ def test_smooth_pair_equals_two_sweeps_bit_for_bit(agd, ctx, grad, shape, store,
 
 TWO_SHAPES = [((3001, 1024), "f32"), ((2000, 512), "f32"), ((501, 1001), "f32"), ((1500, 512), "f64"), ((700, 300), "f64"),
               ((16, 1024), "f32"), ((9, 640), "f32"), ((1200, 1024), "f64"), ((900, 2048), "f32"), ((333, 1500), "f32"),
-              ((2000, 1024), "bf16"), ((517, 4096), "bf16"), ((300, 128), "bf16")]     # tcgen05: r at w2 rides in B columns 3-5
+              ((2000, 1024), "bf16"), ((517, 4096), "bf16"), ((300, 128), "bf16"), ((700, 768), "bf16"), ((260, 640), "bf16")]     # wgmma: r at w2 rides in B columns of its own
 
 
 @pytest.mark.parametrize("grad", GRADS)
@@ -497,7 +496,7 @@ def test_smooth_two_unsupported_shards_refuse(agd, ctx):
     rng = np.random.default_rng(5)
     X = rng.standard_normal((300, 4096)).astype(np.float32)
     y = (rng.random(300) > 0.5).astype(np.float64)
-    for store, dd in (("f32", 4096), ("bf16", 1024)):        # four vectors per thread / tcgen05 with fp64 margins: no two-gradient form
+    for store, dd in (("f32", 4096), ("bf16", 1024)):        # four vectors per thread / wgmma with fp64 margins: no two-gradient form
         ds = ctx.parallelize(y, X[:, :dd].copy(), store=store)
         if store == "bf16":
             ds.set_option("tc_margins", "f64")
@@ -515,7 +514,7 @@ SPEC_CASES = [(20000, 1024, "logistic", "simple", 0.0, "f32", 12, {}),
               (4000, 256, "least_squares", "simple", 0.0, "f64", 25, {"L0": 1e-3}),                 # L-increase: guesses rejected
               (1000, 100, "least_squares", "squared_l2", 0.1, "f64", 30, {}),                       # restarts: (f_x, g_x) reused
               (1000, 512, "least_squares", "simple", 0.0, "f64", 60, {"tol": 1e-6}),               # leaves through :322-324
-              (5000, 1024, "logistic", "simple", 0.0, "bf16", 8, {}),                               # tcgen05 kernel, two-gradient form
+              (5000, 1024, "logistic", "simple", 0.0, "bf16", 8, {}),                               # wgmma kernel, two-gradient form
               (3000, 4096, "least_squares", "squared_l2", 0.01, "bf16", 8, {})]
 
 
@@ -566,7 +565,7 @@ def test_smooth_pair_csr_and_unsupported_kernels(agd, ctx, oracle):
     # kernels without a two-point form refuse (agd_run then simply does not fuse)
     X = rng.standard_normal((300, 1024)).astype(np.float32)
     yd = (rng.random(300) > 0.5).astype(np.float64)
-    ds = ctx.parallelize(yd, X, store="bf16")                   # tcgen05 path: only its default (fp32-margin) mapping has one
+    ds = ctx.parallelize(yd, X, store="bf16")                   # wgmma path: only its default (fp32-margin) mapping has one
     ds.set_option("tc_margins", "f64")
     with pytest.raises(agd.NativeError, match="two-point"):
         ds.smooth_pair(agd.LogisticGradient(), np.zeros(1024), np.zeros(1024))
@@ -586,9 +585,9 @@ FUSE_CASES = [(20000, 1024, "logistic", "simple", 0.0, "f32", 12, {}),
               (4000, 300, "logistic", "simple", 0.0, "f64", 20, {"beta": 1.0, "L0": 0.25, "Lexact": 0.25, "may_restart": False}),
               (3000, 20000, "logistic", "squared_l2", 0.01, "f32", 8, {}),                    # generic kernel
               (1000, 512, "least_squares", "simple", 0.0, "f64", 60, {"tol": 1e-6}),          # leaves through :322-324
-              (6000, 1024, "least_squares", "squared_l2", 0.01, "bf16", 10,                     # tcgen05 kernel, branch-free config
+              (6000, 1024, "least_squares", "squared_l2", 0.01, "bf16", 10,                     # wgmma kernel, branch-free config
                {"beta": 1.0, "L0": 8.0, "Lexact": 8.0, "may_restart": False}),
-              (5000, 4096, "logistic", "simple", 0.0, "bf16", 8, {})]                           # tcgen05 kernel, defaults
+              (5000, 4096, "logistic", "simple", 0.0, "bf16", 8, {})]                           # wgmma kernel, defaults
 
 
 @pytest.mark.parametrize("case", FUSE_CASES, ids=[f"{c[0]}x{c[1]}-{c[2]}-{c[3]}-{i}" for i, c in enumerate(FUSE_CASES)])
