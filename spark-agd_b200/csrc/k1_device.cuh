@@ -18,7 +18,8 @@ __device__ __forceinline__ double log1p_exp(double x) { return x > 0 ? x + log1p
 // with  exp: 32-entry 2^(j/32) table + degree-7 polynomial (Estrin), Cody-Waite reduction;
 //       1/u: rcp.approx seed + 2 Newton steps;  log(u): fdlibm's s = f/(2+f) series, Estrin form.
 // The q and log chains are independent, so one lane overlaps them.  Accuracy ~2 ulp (4e-16 relative
-// on both outputs against a long-double evaluation; libm: 2.6e-16) -- see tests/test_gpu_parity.py.
+// on both outputs against a long-double evaluation; libm: 2.6e-16) -- see tests/test_gpu_parity.py; e is right
+// into the subnormals (|margin| up to 745.13, then 0), checked row by row in tests/test_k1_exact.py.
 static __device__ const double kExp2Tab[32] = {
     1.0, 1.0218971486541166, 1.0442737824274138, 1.0671404006768237, 1.0905077326652577, 1.1143867425958924,
     1.1387886347566916, 1.1637248587775775, 1.189207115002721, 1.215247359980469, 1.2418578120734840,
@@ -59,8 +60,12 @@ __device__ __forceinline__ double logistic_head(double m, double y, LogisticMid 
   const double em1 = fma(r2, S, r);
   const double T = kExp2Tab[n & 31];
   double e = fma(T, em1, T);
-  e *= __longlong_as_double((long long)((n >> 5) + 1023) << 52);
-  if (a > 700.0) e = 0.0;
+  // 2^(n >> 5) in two exact steps: one factor would leave the normal range below a ~ 708.4, while the product rounds once,
+  // into the subnormals, down to the underflow point a ~ 745.13 (above 746 the reduction itself is out of range)
+  const int k1 = (n >> 5) >> 1, k2 = (n >> 5) - k1;
+  e *= __longlong_as_double((long long)(k1 + 1023) << 52);
+  e *= __longlong_as_double((long long)(k2 + 1023) << 52);
+  if (a > 746.0) e = 0.0;
   if (a != a) e = a;  // NaN margin propagates, as it does through Math.exp
   const double u = 1.0 + e;
   const double q = rcp_1to4(u);

@@ -17,8 +17,10 @@
 // ring of groups of gb blocks of [16 rows][64 features] (gb = the largest even divisor of d / 64 that is <= 8, so a tile is
 // a whole number of groups for every role); a group is released once the wgmmas reading it
 // have completed in all four MMA warps.
-// Accuracy: the gradient carries the bf16x3 split (2^-24) and fp32 sums over 16 rows, i.e. ~1e-7 relative
-// (tests/test_gpu_parity.py states the bound).
+// Accuracy (per element; DESIGN.md section 4, tests/k1_reference.py): |dg_j| <= [sum_i |x_ij| (lambda eps_i + 2^-20 |r_i|)] / n
+// (+ rows at the hinge kink), eps_i = 2^-20 sum_j |x_ij w_j| with fp32 margins.  r of each tile is scaled by a power of two
+// before the split, so this holds for every finite r while |x| <= 2^100; fp32 margins need |x_ij w_j| and their partial
+// sums inside fp32's exponent range.  Measured on an H100 80GB HBM3 at 400 W: at most 0.064 of the gradient bound.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -39,6 +41,7 @@ constexpr int kKR = 16;            // rows per tile = K of one MMA
 constexpr int kRegsConsumer = 64, kRegsAux = 56, kRegsMma = 168;
 constexpr int kBlockBytes = kKR * 128;     // one [16 rows][64 features] swizzled block
 constexpr int kBBytes = 1024;              // one B operand buffer: [N <= 24 columns][16 rows] bf16, K-major, no swizzle
+constexpr int kScaleOff = 768;             // ... followed by the tile's scale factor 2^s per point (2 doubles), which no MMA reads
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -111,10 +114,12 @@ __device__ __forceinline__ void wgmma_bf16<24>(float (&d)[12], uint64_t adesc, u
                : "memory");
 }
 
-// MMA warpgroup: adds the owned feature's hi + mid + lo (and hi2 + mid2 + lo2) of a 128-feature pair into fp64.  Fragment
-// index for row-half 0 (row-half 1: + 2): hi 0, mid 1, lo 4, hi2 5, mid2 8, lo2 9.
+// MMA warpgroup: adds the owned feature's hi + mid + lo (and hi2 + mid2 + lo2) of a 128-feature pair into fp64, undoing the
+// tile's power-of-two scaling of r (sc[0] = 2^s; sc[1] at the second point).  Fragment index for row-half 0
+// (row-half 1: + 2): hi 0, mid 1, lo 4, hi2 5, mid2 8, lo2 9.
 template <int N, bool TWO>
-__device__ __forceinline__ void mma_accumulate(const float (&e)[2][N / 2], int hb, int hs, double &g, double *g2) {
+__device__ __forceinline__ void mma_accumulate(const float (&e)[2][N / 2], int hb, int hs, const double (&sc)[2], double &g,
+                                               double *g2) {
   float v[6];
 #pragma unroll
   for (int t = 0; t < (TWO ? 6 : 3); ++t) {
@@ -122,9 +127,11 @@ __device__ __forceinline__ void mma_accumulate(const float (&e)[2][N / 2], int h
     const float x0 = hs ? e[0][i + 2] : e[0][i], x1 = hs ? e[1][i + 2] : e[1][i];
     v[t] = hb ? x1 : x0;
   }
-  g += ((double)v[0] + (double)v[1]) + (double)v[2];
-  if (TWO) *g2 += ((double)v[3] + (double)v[4]) + (double)v[5];
+  g += (((double)v[0] + (double)v[1]) + (double)v[2]) * sc[0];
+  if (TWO) *g2 += (((double)v[3] + (double)v[4]) + (double)v[5]) * sc[1];
 }
+// 2^k for -1022 <= k <= 1023
+__device__ __forceinline__ double pow2i(int k) { return __longlong_as_double((long long)(k + 1023) << 52); }
 // the ring group may be refilled once all four MMA warps are done with it
 __device__ __forceinline__ void mma_release(uint32_t empty_bar, int lane) {
   __syncwarp();
@@ -294,13 +301,31 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
         }
       }
       named_arrive(3 + bb, kConsumers + 32);                   // partial[bb] may be overwritten
+      // r of the tile is split after scaling by 2^-s, s = the exponent of max |r| over its 16 rows (per point): the pieces
+      // and the fp32 sums then stay in range for every finite r as long as |x| <= 2^100 (16 x 2^100 < 2^127).  Scaling by a
+      // power of two is exact, so in-range tiles give the bits of the unscaled split.
+      // The largest exponent field of the tile (high word of |r|, one warp reduction per point) gives s with
+      // max |r| 2^-s in [0.5, 1): s = E - 1022; a subnormal maximum takes s = -1022, inf / NaN s = 0.
+      const uint32_t hw = (uint32_t)__double2hiint(mult) & 0x7fffffffu;
+      uint32_t E = __reduce_max_sync(0xffffffffu, lane < kKR ? hw : 0u) >> 20;
+      if (DUAL == 2) {
+        const uint32_t E2 = __reduce_max_sync(0xffffffffu, lane < kKR ? 0u : hw) >> 20;
+        if (second) E = E2;
+      }
+      // (s = 1024 is taken as 1023, max |r| 2^-s in [1, 2): then 2^s is a normal double and one DMUL undoes it)
+      const int s = E == 0x7ffu ? 0 : E == 0u ? -1022 : E == 0x7feu ? 1023 : (int)E - 1022;
+      const int ns = -s;
+      const double ms = (mult * pow2i(ns >> 1)) * pow2i(ns - (ns >> 1));
       if (k >= 2) mbar_wait(b2_empty + 8u * bb, (uint32_t)(((k >> 1) - 1) & 1));  // MMAs of tile k-2 have read b2[bb]
+      if (srow == 0 && (lane < kKR || (DUAL == 2 && second))) {
+        reinterpret_cast<double *>(b2 + bb * kBBytes + kScaleOff)[second ? 1 : 0] = pow2i(s);
+      }
       if (lane < kKR || (DUAL == 2 && second)) {
-        // r_i -> three bf16 pieces, each written to four columns of the K-major B operand: element (n, row) sits at
+        // r_i 2^-s -> three bf16 pieces, each written to four columns of the K-major B operand: element (n, row) sits at
         // (n / 8) * 256 + (row / 8) * 128 + (n % 8) * 16 + (row % 8) * 2.  At w: hi -> 2t, mid -> 2t+1, lo -> 8+2t;
         // at w2: hi2 -> 9+2t, mid2 -> 16+2t, lo2 -> 17+2t (t = 0..3)
-        const __nv_bfloat16 hi = __double2bfloat16(mult);
-        const double r1 = mult - (double)__bfloat162float(hi);
+        const __nv_bfloat16 hi = __double2bfloat16(ms);
+        const double r1 = ms - (double)__bfloat162float(hi);
         const __nv_bfloat16 mid = __double2bfloat16(r1);
         const double r2 = r1 - (double)__bfloat162float(mid);
         const __nv_bfloat16 lo = __double2bfloat16(r2);
@@ -356,6 +381,8 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
       const int bb = (int)(k & 1);
       mbar_wait(b2_full + 8u * bb, (uint32_t)((k >> 1) & 1));
       const uint64_t bdesc = gmma_desc(smem_u32(b2 + bb * kBBytes), 128, 256, 0);   // K-major, no swizzle
+      const double *scs = reinterpret_cast<const double *>(b2 + bb * kBBytes + kScaleOff);
+      const double sc[2] = {scs[0], DUAL == 2 ? scs[1] : 1.0};
 #pragma unroll
       for (int p = 0; p < 32; ++p) {
         if (p < npairs) {
@@ -374,7 +401,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
           }
           wgmma_commit();
           wgmma_wait<0>();
-          mma_accumulate<kN, DUAL == 2>(acc, hb, hs, gacc[p], g2 + 128 * p + fo);
+          mma_accumulate<kN, DUAL == 2>(acc, hb, hs, sc, gacc[p], g2 + 128 * p + fo);
           if (pg == hp - 1) mma_release(bars + 8u * (RG + slot), lane);   // last pair of the group
         }
       }

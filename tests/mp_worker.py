@@ -78,6 +78,22 @@ def main():
     ws, hs, ss = S.run_with_stats(syn, S.LogisticGradient(), S.SimpleUpdater(), 0.0, 5, 0.0, np.zeros(512))
     res["synthetic"] = {"w": ws.tolist(), "hist": hs.tolist(), "passes": ss.passes, "rows_local": syn.local_rows(0)}
     syn.close()
+    # mini-batch runs on bf16 shards through the wgmma kernel: the row mask is keyed by the global row id, so every rank
+    # but 0 needs its shard's row_base.  Generated in place: rank r's rows start at r * n / W (the oracle's row ids);
+    # loaded: rank r's rows are numbered from r << 40
+    synb = ctx.synthetic(20000, 512, S.LogisticGradient(), seed=42, store="bf16")
+    synb.set_option("k1_variant", "tc")
+    wb, hb = S.GradientDescent.runMiniBatchSGD(synb, S.LogisticGradient(), S.SquaredL2Updater(), 0.5, 8, 0.01, 0.25, np.zeros(512))
+    labels = [None] * world
+    dist.all_gather_object(labels, synb.get_labels(0, 0, synb.local_rows(0)).tolist())
+    res["minibatch_bf16_synthetic"] = {"w": wb.tolist(), "hist": hb.tolist(), "labels": sum(labels, [])}
+    synb.close()
+    lo, hi = rank * n // world, (rank + 1) * n // world
+    ldb = ctx.parallelize(y[lo:hi], X[lo:hi], store="bf16")
+    ldb.set_option("k1_variant", "tc")
+    wl, hl = S.GradientDescent.runMiniBatchSGD(ldb, S.LogisticGradient(), S.SimpleUpdater(), 0.5, 6, 0.0, 0.25, np.zeros(d))
+    res["minibatch_bf16_loaded"] = {"w": wl.tolist(), "hist": hl.tolist()}
+    ldb.close()
     # a wide sparse shard: d + 4 = 100004 doubles per sweep takes the reduce-scatter + all-gather form of the exchange
     n3, d3, k3 = 9000, 100000, 12
     rp, ix, va, y3 = make_csr(n3, d3, k3, 13)

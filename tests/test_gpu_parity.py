@@ -3,8 +3,14 @@
 Tolerances: the element-wise vector arithmetic is bit-faithful; reductions differ only in fp64
 summation order, so losses agree to ~1e-13 relative and trajectories (weights after equal
 iterations) to <= 1e-9 relative -- far inside north_star's 1e-5 bound, which is also asserted."""
+import os
+import sys
+
 import numpy as np
 import pytest
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import k1_reference as R  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -186,17 +192,30 @@ def tc_shape(d):
     return d % 128 == 0 and d <= 4096
 
 
+def assert_within_tc_bounds(record_property, grad, Xs, y, w, f32_margins, loss, g, ref_loss, ref_g):
+    """The wgmma kernel's element-wise contract (tests/k1_reference.py): every gradient entry and the loss within the bound
+    that the margin error (fp32 margins: 2^-20 sum |x w|) and the bf16 x 3 split with fp32 tile sums (2^-20 sum |x r|) allow."""
+    gb, lb, _ = R.dense_bounds(grad, Xs, y, w, f32_margins=f32_margins)
+    eg, el = float(np.max(np.abs(g - ref_g) / gb)), abs(loss - ref_loss) / lb
+    record_property("grad_normwise", rel_err(g, ref_g))
+    record_property("loss_rel", abs(loss - ref_loss) / abs(ref_loss))
+    record_property("grad_elementwise_of_bound", eg)
+    record_property("loss_of_bound", el)
+    assert eg <= 1.0 and el <= 1.0, (eg, el)
+
+
 @pytest.mark.parametrize("variant", ["auto", "auto-f64", "ring"])
 @pytest.mark.parametrize("grad", ["logistic", "least_squares", "hinge"])
 @pytest.mark.parametrize("shape", [(3001, 1024), (2000, 512), (515, 256), (777, 2048), (300, 4096), (129, 1104),
                                    (37, 40), (10, 20000), (64, 8192), (5, 3), (4099, 128), (33, 3072), (517, 768),
                                    (260, 640)])
-def test_bf16_storage_matches_oracle(agd, ctx, oracle, grad, shape, variant):
+def test_bf16_storage_matches_oracle(agd, ctx, oracle, record_property, grad, shape, variant):
     """X stored as bf16 in HBM (rounded to nearest-even at load).  `ring`/generic: fp64 CUDA-core path, same
     tolerances as fp32 storage.  `auto` on d % 128 == 0, d <= 4096 is the wgmma kernel: X^T r on the tensor cores with r
-    split into three bf16 pieces and fp32 partial sums over 16 rows -> gradient to 2e-6; margins on the CUDA cores, by
-    default in fp32 (w rounded to fp32, packed FMAs over at most 8 terms, then fp64) -> loss to 2e-6, or fp64-exact with
-    option tc_margins=f64 (`auto-f64`) -> loss to 1e-12.  Off the tensor path `auto-f64` checks that the option changes
+    split into three bf16 pieces and fp32 partial sums over 16 rows -> gradient to 3e-7 norm-wise and within the
+    element-wise bound of tests/k1_reference.py; margins on the CUDA cores, by default in fp32 (w rounded to fp32, packed
+    FMAs over at most 8 terms, then fp64) -> loss to 1.5e-7, or fp64-exact with option tc_margins=f64 (`auto-f64`) -> loss
+    to 1e-12.  Off the tensor path `auto-f64` checks that the option changes
     nothing, and `ring` forces the generic CUDA-core kernel (auto takes the ring wherever the ring fits)."""
     n, d = shape
     rng = np.random.default_rng(3000 + n + d)
@@ -214,8 +233,10 @@ def test_bf16_storage_matches_oracle(agd, ctx, oracle, grad, shape, variant):
     ref_loss, ref_g, _ = oracle.smooth(oracle.Data(y, X=Xs), grad, w, partitions=2)
     assert cnt == n
     tensor_path = variant != "ring" and tc_shape(d)
-    np.testing.assert_allclose(loss, ref_loss, rtol=2e-6 if (tensor_path and variant == "auto") else 1e-12)
-    assert rel_err(g, ref_g) < (3e-6 if tensor_path else 1e-12)
+    np.testing.assert_allclose(loss, ref_loss, rtol=1.5e-7 if (tensor_path and variant == "auto") else 1e-12)
+    assert rel_err(g, ref_g) < (3e-7 if tensor_path else 1e-12)
+    if tensor_path:
+        assert_within_tc_bounds(record_property, grad, Xs, y, w, variant == "auto", loss, g, ref_loss, ref_g)
     a = ds.smooth(G(agd, grad), w)
     assert a[0] == loss and np.array_equal(a[1], g)      # deterministic either way
     ds.close()
@@ -224,7 +245,7 @@ def test_bf16_storage_matches_oracle(agd, ctx, oracle, grad, shape, variant):
 @pytest.mark.parametrize("rows_opt,copy_opt", [(0, 0), (0, 2), (1, 0), (1, 2), (4, 0), (4, 2)])
 @pytest.mark.parametrize("shape,grad", [((3001, 1024), "logistic"), ((300, 4096), "least_squares"), ((515, 256), "hinge"),
                                         ((1000, 128), "logistic"), ((130, 3072), "least_squares"), ((517, 768), "hinge")])
-def test_tc_kernel_forms(agd, ctx, oracle, shape, grad, rows_opt, copy_opt):
+def test_tc_kernel_forms(agd, ctx, oracle, record_property, shape, grad, rows_opt, copy_opt):
     """The wgmma kernel's consumer mappings (ring_rows: 0 = default, two rows per thread of the column-slice mapping; 4 = four
     rows per thread; 1 = row per lane with broadcast w reads) and its two TMA forms (default: one 3-D copy per ring group;
     ring_ctas=2: one 2-D copy per 64-feature block) all meet the tolerances of the tensor path."""
@@ -240,8 +261,9 @@ def test_tc_kernel_forms(agd, ctx, oracle, shape, grad, rows_opt, copy_opt):
     loss, g, cnt = ds.smooth(G(agd, grad), w)
     ref_loss, ref_g, _ = oracle.smooth(oracle.Data(y, X=agd.bf16_to_f32(raw)), grad, w, partitions=2)
     assert cnt == n
-    np.testing.assert_allclose(loss, ref_loss, rtol=2e-6 if rows_opt == 0 else 1e-12)   # default mapping: fp32 margins
-    assert rel_err(g, ref_g) < 3e-6
+    np.testing.assert_allclose(loss, ref_loss, rtol=1.5e-7 if rows_opt == 0 else 1e-12)   # default mapping: fp32 margins
+    assert rel_err(g, ref_g) < 3e-7
+    assert_within_tc_bounds(record_property, grad, agd.bf16_to_f32(raw), y, w, rows_opt == 0, loss, g, ref_loss, ref_g)
     ds.close()
 
 
@@ -382,25 +404,40 @@ def test_suite_T1_T2_T4_on_gpu(agd, ctx, oracle, fixture_gd_input):
 
 
 @pytest.mark.parametrize("shape,store,variant", [((20000, 1024), "f32", "auto"), ((5000, 100), "f64", "auto"),
-                                                 ((9000, 512), "f32", "ring"), ((3000, 30), "f64", "auto")])
+                                                 ((9000, 512), "f32", "ring"), ((3000, 30), "f64", "auto"),
+                                                 ((3001, 1024), "bf16", "tc"), ((3001, 1024), "bf16", "ring"),
+                                                 ((3000, 1024), "f64", "generic"), ((3000, 700), "csr-f32", "auto"),
+                                                 ((3000, 700), "csr-f64", "auto")])
 @pytest.mark.parametrize("fraction", [0.25, 0.9])
 def test_minibatch_gd_matches_oracle(agd, ctx, oracle, shape, store, variant, fraction):
-    """SURVEY.md 8(f).1: GradientDescent.runMiniBatchSGD with miniBatchFraction < 1 on the same kernels (row mask +
-    selected-row count through the slabs), against the oracle's restatement with the same counter-based mask."""
+    """SURVEY.md 8(f).1: GradientDescent.runMiniBatchSGD with miniBatchFraction < 1 on every gradient kernel (row mask +
+    selected-row count through the slabs: wgmma, ring, generic, CSR), against the oracle's restatement with the same
+    counter-based mask.  The wgmma kernel is held to its own accuracy (fp32 margins, bf16 x 3 split)."""
     n, d = shape
     rng = np.random.default_rng(500 + n + d)
-    X, y = make_data(rng, n, d, "logistic", np.float32 if store == "f32" else np.float64)
+    X, y = make_data(rng, n, d, "logistic", np.float64 if store == "f64" or store == "csr-f64" else np.float32)
     w0 = rng.standard_normal(d) * 0.01
-    data = ctx.parallelize(y, X, store=store)
+    if store.startswith("csr"):
+        keep = np.abs(X) > 1.0                                      # about a third of the entries
+        rowptr = np.concatenate([[0], np.cumsum(keep.sum(axis=1))]).astype(np.int64)
+        idx = np.nonzero(keep)[1].astype(np.int32)
+        D = oracle.Data(y, csr=(rowptr, idx, X[keep]), d=d)
+        data = ctx.parallelize_csr(y, rowptr, idx, X[keep], d, store=store[4:])
+    else:
+        if store == "bf16":
+            X = R.bf16_to_f32(R.f32_to_bf16_bits(X))
+        D = oracle.Data(y, X=X)
+        data = ctx.parallelize(y, X, store=store)
     if variant != "auto":
         data.set_option("k1_variant", variant)
     w, hist = agd.GradientDescent.runMiniBatchSGD(data, agd.LogisticGradient(), agd.SquaredL2Updater(), 0.5, 12, 0.01,
                                                   fraction, w0)
-    rw, rh = oracle.gd_run(oracle.Data(y, X=X), "logistic", "squared_l2", w0, step_size=0.5, num_iterations=12,
+    rw, rh = oracle.gd_run(D, "logistic", "squared_l2", w0, step_size=0.5, num_iterations=12,
                            reg_param=0.01, mini_batch_fraction=fraction)
     assert len(hist) == len(rh) == 12
-    np.testing.assert_allclose(hist, rh, rtol=1e-11)
-    assert rel_err(w, rw) < 1e-10
+    tc = variant == "tc"
+    np.testing.assert_allclose(hist, rh, rtol=1e-7 if tc else 1e-11)
+    assert rel_err(w, rw) < (1e-6 if tc else 1e-10)
     full = agd.GradientDescent.runMiniBatchSGD(data, agd.LogisticGradient(), agd.SquaredL2Updater(), 0.5, 12, 0.01, 1.0, w0)
     assert not np.allclose(full[1], hist)          # the mask really drops rows
     data.close()

@@ -16,6 +16,7 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from k1_reference import bf16_to_f32, f32_to_bf16_bits, row_selected, row_terms  # noqa: E402
 from mp_worker import make_csr, make_data  # noqa: E402
 
 
@@ -103,6 +104,26 @@ def test_process_per_rank_world_matches_oracle(oracle, tmp_path, transport, worl
     np.testing.assert_allclose(res["synthetic"]["hist"], refs.loss_history, rtol=1e-11)
     assert np.linalg.norm(np.array(res["synthetic"]["w"]) - refs.weights) <= 1e-9 * np.linalg.norm(refs.weights)
     assert res["synthetic"]["passes"] == refs.passes
+    # --- mini-batch runs on bf16 shards (wgmma kernel): every rank but 0 samples with row_base != 0
+    mb = res["minibatch_bf16_synthetic"]
+    Xb = bf16_to_f32(f32_to_bf16_bits(Xs))
+    rw, rh = O.gd_run(O.Data(np.array(mb["labels"]), X=Xb), "logistic", "squared_l2", np.zeros(512), step_size=0.5,
+                      num_iterations=8, reg_param=0.01, partitions=world, threads=world, mini_batch_fraction=0.25)
+    assert len(mb["hist"]) == len(rh) == 8
+    np.testing.assert_allclose(mb["hist"], rh, rtol=1e-7)
+    assert np.linalg.norm(np.array(mb["w"]) - rw) <= 1e-6 * np.linalg.norm(rw)
+    # loaded shards number rank r's rows from r << 40: fp64 restatement of the same loop with that mask
+    ml = res["minibatch_bf16_loaded"]
+    Xl = bf16_to_f32(f32_to_bf16_bits(X)).astype(np.float64)
+    ids = np.concatenate([(r << 40) + np.arange((r + 1) * 6001 // world - r * 6001 // world) for r in range(world)])
+    wr, hr = np.zeros(1024), []
+    for i in range(1, 7):
+        sel = row_selected(42 + i, int(np.ldexp(0.25, 64)), ids)
+        mult, lo = row_terms("logistic", Xl[sel] @ wr, y[sel])
+        hr.append(lo.sum() / sel.sum())
+        wr = wr - 0.5 / np.sqrt(i) * (Xl[sel].T @ mult / sel.sum())
+    np.testing.assert_allclose(ml["hist"], hr, rtol=1e-7)
+    assert np.linalg.norm(np.array(ml["w"]) - wr) <= 1e-6 * np.linalg.norm(wr)
     # --- a wide sparse shard (d = 100000): the exchange takes its reduce-scatter + all-gather form (n >= 32768 doubles)
     rp, ix, va, y3 = make_csr(9000, 100000, 12, 13)
     D3 = O.Data(y3, csr=(rp, ix.ravel(), va.ravel()), d=100000)
