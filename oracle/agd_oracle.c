@@ -83,7 +83,11 @@ static inline double row_dot(const oracle_data *D, int64_t i, const double *w) {
   }
   return s;
 }
+/* Dense axpy is netlib DAXPY (through F2J), which starts with IF (DA.EQ.0) RETURN: a dense row with multiplier exactly 0 adds
+   nothing, whatever its features.  The sparse axpy of BLAS.scala is a plain loop with no such test, so 0 * inf = NaN shows.
+   On finite rows the return only drops +-0 terms, and a sum that starts at +0 never becomes -0: the bits are the same. */
 static inline void row_axpy(const oracle_data *D, int64_t i, double a, double *g) {
+  if (D->storage != ORACLE_CSR && a == 0.0) return;
   if (D->storage == ORACLE_DENSE_F64) {
     const double *x = D->Xd + i * D->ld;
     for (int32_t j = 0; j < D->d; ++j) g[j] += a * x[j];

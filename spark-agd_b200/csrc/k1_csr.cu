@@ -17,6 +17,13 @@ namespace agd {
 
 namespace {
 
+// Which rows reach the scatter.  The sparse BLAS.axpy [mllib-1.3.0] is a plain loop with no zero test, so a row the sample
+// keeps adds mult * x even when mult is exactly 0 (0 * inf = NaN must show); only a hinge row outside the margin, for which
+// HingeGradient never calls axpy, adds nothing.  A hinge row inside the margin has mult = -+1, never 0.
+__device__ __forceinline__ bool csr_row_folds(int kind, bool sel, double mult) {
+  return sel && (mult != 0.0 || kind != AGD_GRAD_HINGE);
+}
+
 template <typename T, bool DUAL>
 __global__ void __launch_bounds__(256) k1_csr_kernel(const K1CsrArgs a) {
   __shared__ double red[32];
@@ -50,7 +57,7 @@ __global__ void __launch_bounds__(256) k1_csr_kernel(const K1CsrArgs a) {
       loss_eval(a.kind, m2, ylab, mult2, loss2);
       lossacc2 += loss2;
     }
-    if (mult != 0.0) {
+    if (csr_row_folds(a.kind, sel, mult)) {
       for (long long k = lo + lane; k < hi; k += 32) atomicAdd(&a.gacc[a.idx[k]], mult * (double)val[k]);
     }
   }
@@ -133,7 +140,7 @@ __global__ void __launch_bounds__(256) k1_csr_pipelined_kernel(const K1CsrArgs a
       loss_eval(a.kind, m2, ylab, mult2, loss2);
       lossacc2 += loss2;
     }
-    if (mult != 0.0) {
+    if (csr_row_folds(a.kind, sel, mult)) {
       if (h0) atomicAdd(&a.gacc[c0], mult * x0);
       if (h1) atomicAdd(&a.gacc[c1], mult * x1);
       for (long long k = k1 + 32; k < hi; k += 32) atomicAdd(&a.gacc[a.idx[k]], mult * (double)val[k]);

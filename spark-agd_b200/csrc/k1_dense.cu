@@ -100,7 +100,7 @@ __host__ __device__ inline uint32_t round_up_u32(uint32_t v, uint32_t a) { retur
 
 // shared-memory carve-up (identical on host and device)
 struct RingLayout {
-  uint32_t stage_stride, aux_off, partial_off, partial2_off, mult_off, mult2_off, red_off, cnt_off, bars_off, total;
+  uint32_t stage_stride, aux_off, partial_off, partial2_off, mult_off, mult2_off, red_off, cnt_off, skip_off, bars_off, total;
 };
 // mode: 0 = one point; 1 = the launch also evaluates the LOSS at a second point w2 (pass fusion of the history evaluation);
 // 2 = loss AND gradient at w2 (the speculative sweep of the memoised pass structure).  aux holds w (and w2) in the
@@ -115,7 +115,8 @@ __host__ __device__ inline RingLayout ring_layout(uint32_t tile_bytes, uint32_t 
   L.mult2_off = L.mult_off + kMaxTileRows * 8;
   L.red_off = L.mult2_off + (mode == 2 ? kMaxTileRows * 8 : 0);
   L.cnt_off = L.red_off + 32 * 8;
-  L.bars_off = L.cnt_off + round_up_u32(stages * 4, 8);
+  L.skip_off = L.cnt_off + round_up_u32(stages * 4, 8);
+  L.bars_off = L.skip_off + 8;
   L.total = L.bars_off + (stages + 1) * 8;
   return L;
 }
@@ -177,6 +178,7 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
   double *mult2_s = reinterpret_cast<double *>(smem + L.mult2_off);    // [TR] at w2 (MODE 2)
   double *red = reinterpret_cast<double *>(smem + L.red_off);
   unsigned int *cnt = reinterpret_cast<unsigned int *>(smem + L.cnt_off);  // [S] warps done with the stage (diagnostic modes)
+  uint32_t *skip_s = reinterpret_cast<uint32_t *>(smem + L.skip_off);      // the tile's rows that must add nothing (below)
   const uint32_t bars = smem_u32(smem + L.bars_off);                   // full[s] = bars + 8*s ; wbar = bars + 8*S
   const uint32_t wbar = bars + 8u * S;
   const unsigned char *Xb = reinterpret_cast<const unsigned char *>(a.X);
@@ -411,38 +413,60 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
       double mult, loss = 0.0;
       if (a.kind == AGD_GRAD_LOGISTIC) mult = logistic_head(m, ylab, mid);
       else loss_eval(a.kind, m, ylab, mult, loss);
-      if (DUAL ? lane < 16 : srow < TR) mult_s[srow] = row_ok ? mult : 0.0;
-      if (MODE == 2 && lane >= 16) mult2_s[srow] = row_ok ? mult : 0.0;
+      const double mw = row_ok ? mult : 0.0;
+      if (DUAL ? lane < 16 : srow < TR) mult_s[srow] = mw;
+      if (MODE == 2 && lane >= 16) mult2_s[srow] = mw;
       if (a.kind != AGD_GRAD_LOGISTIC) lossacc += row_ok ? loss : 0.0;
       cntacc += row_ok ? 1.0 : 0.0;
+      // A row whose multiplier is exactly 0 adds nothing (netlib DAXPY returns when DA == 0), but 0 * inf is NaN.  Flag the
+      // rows where that can happen: a finite margin means every feature of the row is finite (padded columns are zero).
+      // Bit = tile row; with a second gradient (MODE 2), bits 16 + row are the rows at w2.
+      const bool poison = srow < rv && (!DUAL || MODE == 2 || lane < 16) && mw == 0.0 && !isfinite(m);
+      const uint32_t flagged_rows = __ballot_sync(0xffffffffu, poison);
+      if (lane == 0) *skip_s = flagged_rows;
     }
     __syncthreads();
 
-    // phase 2: g += mult_i * x_i on the retained fp64 tile
-    auto phase2 = [&]() {
+    // phase 2: g += mult_i * x_i on the retained fp64 tile.  Flagged rows (rare: non-finite features) must leave the sums as
+    // they are.  With one gradient their retained x is zeroed, which only turns +-0 or NaN terms into +0; with two, the FMAs
+    // are select-guarded, one guard per point.
+    const uint32_t skip = *skip_s;
+    auto fold = [&](const double *ms, double (&av)[V][EPV], uint32_t flagged) {
       double mu[R];
 #pragma unroll
-      for (int r = 0; r < R; ++r) mu[r] = mult_s[g * R + (r ^ rperm)];
-#pragma unroll
-      for (int r = 0; r < R; ++r) {
-#pragma unroll
-        for (int v = 0; v < V; ++v)
-#pragma unroll
-          for (int e = 0; e < EPV; ++e) acc[v][e] = fma(mu[r], xd[r][v][e], acc[v][e]);
-      }
-      if (MODE == 2) {   // the gradient at w2 from the same retained tile
-#pragma unroll
-        for (int r = 0; r < R; ++r) mu[r] = mult2_s[g * R + (r ^ rperm)];
+      for (int r = 0; r < R; ++r) mu[r] = ms[g * R + (r ^ rperm)];
+      if (MODE != 2 || flagged == 0u) {
 #pragma unroll
         for (int r = 0; r < R; ++r)
 #pragma unroll
           for (int v = 0; v < V; ++v)
 #pragma unroll
-            for (int e = 0; e < EPV; ++e) {
-              double &dst = accB[MODE == 2 ? v : 0][MODE == 2 ? e : 0];
-              dst = fma(mu[r], xd[r][v][e], dst);
-            }
+            for (int e = 0; e < EPV; ++e) av[v][e] = fma(mu[r], xd[r][v][e], av[v][e]);
+      } else {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+          const bool keep = ((flagged >> (g * R + (r ^ rperm))) & 1u) == 0u;
+#pragma unroll
+          for (int v = 0; v < V; ++v)
+#pragma unroll
+            for (int e = 0; e < EPV; ++e) av[v][e] = keep ? fma(mu[r], xd[r][v][e], av[v][e]) : av[v][e];
+        }
       }
+    };
+    if (MODE != 2 && skip != 0u) {
+#pragma unroll
+      for (int r = 0; r < R; ++r)
+        if ((skip >> (g * R + (r ^ rperm))) & 1u) {
+#pragma unroll
+          for (int v = 0; v < V; ++v)
+#pragma unroll
+            for (int e = 0; e < EPV; ++e) xd[r][v][e] = 0.0;
+        }
+    }
+    auto phase2 = [&]() {
+      fold(mult_s, acc, MODE == 2 ? (skip & 0xffffu) : skip);
+      if (MODE == 2)   // the gradient at w2 from the same retained tile
+        fold(mult2_s, reinterpret_cast<double (&)[V][EPV]>(accB), skip >> 16);
     };
     if (a.kind == AGD_GRAD_LOGISTIC && warp == sw) {
       // warp-uniform branch: the log chain of the loss (all 32 lanes, lanes >= TR carry don't-care values) is
@@ -586,11 +610,16 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
       lossacc += loss;
     }
     __syncthreads();
+    // a row whose multiplier is exactly 0 adds nothing, whatever its features (netlib DAXPY returns when DA == 0): the test
+    // is uniform over the CTA, and on finite rows it drops only +-0 terms
+    double mu[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) mu[r] = mult_s[r];
     for (int c = tid; c < a.d; c += 256) {
       double sacc = slab[c];
 #pragma unroll
       for (int r = 0; r < R; ++r)
-        if (r < rv) sacc = fma(mult_s[r], load_elem<T>(&X[(size_t)(row0 + r) * a.d + c]), sacc);
+        if (r < rv && mu[r] != 0.0) sacc = fma(mu[r], load_elem<T>(&X[(size_t)(row0 + r) * a.d + c]), sacc);
       slab[c] = sacc;
     }
   }

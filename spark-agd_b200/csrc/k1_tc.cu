@@ -284,6 +284,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
       }
       named_sync(1 + bb, kConsumers + 32);                     // partial dots of tile k are in shared memory
       double mult = 0.0;
+      bool nonfinite = false;   // a non-finite margin at a point whose gradient this launch forms
       if (lane < kKR || second) {
         double m;
         if (RPT) {
@@ -294,6 +295,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
           m = (((pp[0] + pp[1]) + (pp[2] + pp[3])) + ((pp[4] + pp[5]) + (pp[6] + pp[7]))) +
               (((pp[8] + pp[9]) + (pp[10] + pp[11])) + ((pp[12] + pp[13]) + (pp[14] + pp[15])));
         }
+        nonfinite = (lane < kKR || DUAL == 2) && srow < rv && !isfinite(m);
         double mu, loss;
         loss_eval(a.kind, m, ylab, mu, loss);
         if (srow < rv && row_selected(a.sample_seed, a.sample_thresh, a.row_base + tile * kKR + srow)) {
@@ -306,12 +308,42 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
       // power of two is exact, so in-range tiles give the bits of the unscaled split.
       // The largest exponent field of the tile (high word of |r|, one warp reduction per point) gives s with
       // max |r| 2^-s in [0.5, 1): s = E - 1022; a subnormal maximum takes s = -1022, inf / NaN s = 0.
+      // A row whose multiplier is exactly 0 adds nothing (netlib DAXPY returns when DA == 0), but the MMA would form 0 * inf =
+      // NaN from it.  A finite margin means every feature of the row is finite, so only rows with a non-finite margin and
+      // multiplier 0 are flagged, and their 128-byte lines in every group of tile k are zeroed before the MMAs read the tile.
+      // All groups of tile k are still resident: the MMA warps release a group only after reading it, which waits for b2_full.
+      // With a second gradient the tile is shared by both points: only rows flagged at both are zeroed (DESIGN.md section 4).
+      // A non-finite margin rides in bit 31 of the exponent reduction, so tiles without one run no extra warp-wide operation.
       const uint32_t hw = (uint32_t)__double2hiint(mult) & 0x7fffffffu;
-      uint32_t E = __reduce_max_sync(0xffffffffu, lane < kKR ? hw : 0u) >> 20;
-      if (DUAL == 2) {
-        const uint32_t E2 = __reduce_max_sync(0xffffffffu, lane < kKR ? 0u : hw) >> 20;
-        if (second) E = E2;
+      const uint32_t hwf = hw | (nonfinite ? 0x80000000u : 0u);
+      uint32_t top = __reduce_max_sync(0xffffffffu, lane < kKR ? hwf : 0u), top2 = 0u;
+      if (DUAL == 2) top2 = __reduce_max_sync(0xffffffffu, lane < kKR ? 0u : hwf);
+      if ((top | top2) >> 31) {   // rare: the exponents again without the flag, then the rows to zero
+        top = __reduce_max_sync(0xffffffffu, lane < kKR ? hw : 0u);
+        if (DUAL == 2) top2 = __reduce_max_sync(0xffffffffu, lane < kKR ? 0u : hw);
+        const uint32_t fl = __ballot_sync(0xffffffffu, nonfinite && mult == 0.0);
+        const uint32_t zero_rows = DUAL == 2 ? (fl & (fl >> 16) & 0xffffu) : fl;
+        // every role walks the ring in the same order: tile k's groups sit in slots (k ngt + gi) mod RG.  Lane = (block of the
+        // group, 16-byte chunk): the 128B swizzle only permutes the chunks within a row's line.  Rolled loops keep this rare
+        // path from taking registers from the scalar warp's loop (an out-of-line call cost 0.3% of K1 time at d = 1024, H100
+        // 80GB HBM3 at 700 W).
+        const int slot0 = (int)((k * a.ngt) % RG);
+#pragma unroll 1
+        for (uint32_t rows = zero_rows; rows; rows &= rows - 1u) {
+          const int zr = __ffs(rows) - 1;
+          int sl = slot0;
+#pragma unroll 1
+          for (int gi = 0; gi < a.ngt; ++gi) {
+#pragma unroll 1
+            for (int c = lane; c < a.gb * 8; c += 32)
+              *reinterpret_cast<uint4 *>(smem + sl * group_bytes + (c >> 3) * kBlockBytes + zr * 128 + (c & 7) * 16) =
+                  make_uint4(0u, 0u, 0u, 0u);
+            if (++sl == RG) sl = 0;
+          }
+        }
       }
+      uint32_t E = top >> 20;
+      if (DUAL == 2 && second) E = top2 >> 20;
       // (s = 1024 is taken as 1023, max |r| 2^-s in [1, 2): then 2^s is a normal double and one DMUL undoes it)
       const int s = E == 0x7ffu ? 0 : E == 0u ? -1022 : E == 0x7feu ? 1023 : (int)E - 1022;
       const int ns = -s;

@@ -227,3 +227,72 @@ def dense_bounds(kind, X, y, w, f32_margins=True, mask=None):
     gb = (A.T @ (lam * eps + EPS_PIECES * np.abs(r)) + A[kink].sum(axis=0)) / cnt
     lb = np.sum(np.abs(r) * eps + lam * eps ** 2 / 2 + kink * eps) / cnt + 2.0 ** -45 * np.sum(np.abs(loss)) / cnt
     return gb, lb, (loss.sum() / cnt, Xd.T @ r / cnt, cnt)
+
+
+def _exp(x):
+    try:
+        return math.exp(x)
+    except OverflowError:
+        return math.inf
+
+
+def _log1p_exp(x):                                       # MLUtils.log1pExp [mllib-1.3.0]
+    return x + math.log1p(_exp(-x)) if x > 0 else math.log1p(_exp(x))
+
+
+def fold_shard(kind, y, w, X=None, csr=None, sample=None):
+    """The seqOp fold of applySmooth over one shard as the reference performs it, in fp64 with the oracle's order of
+    operations (sequential dot per row, rows folded in order, no FMA): returns (loss sum, row count, gradient sum).
+    X: the stored dense rows (fp32, fp64 or bf16 values); csr: (rowptr, idx, val) as stored.  sample: optional
+    (seed, thresh, global row ids) for the mini-batch mask; rows it drops are never touched.
+    Which rows reach the gradient:
+      dense: the axpy is netlib DAXPY, which returns when the multiplier is exactly 0, so such a row adds nothing whatever
+             its features are (a hinge row outside the margin has multiplier 0 too);
+      CSR:   the sparse axpy has no zero test, so every sampled row adds mult * x (0 * inf = NaN) except a hinge row outside
+             the margin, for which HingeGradient never calls axpy."""
+    w = np.asarray(w, dtype=np.float64)
+    y = np.asarray(y, dtype=np.float64)
+    n, d = len(y), len(w)
+    if X is not None:
+        Xd = np.asarray(X, dtype=np.float64)
+        m = np.zeros(n)
+        with np.errstate(invalid="ignore", over="ignore"):
+            for j in range(d):                           # per row: s += x_j w_j, j ascending
+                m = m + Xd[:, j] * w[j]
+    else:
+        rowptr, idx, val = csr
+        val = np.asarray(val, dtype=np.float64)
+        m = np.zeros(n)
+        for i in range(n):
+            s = 0.0
+            for k in range(int(rowptr[i]), int(rowptr[i + 1])):
+                s += float(val[k]) * float(w[idx[k]])
+            m[i] = s
+    sel = np.ones(n, bool) if sample is None else row_selected(sample[0], sample[1], sample[2])
+    g = np.zeros(d)
+    loss, cnt = 0.0, 0
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(n):
+            if not sel[i]:
+                continue
+            mi, yi = float(m[i]), float(y[i])
+            call = True
+            if kind == "logistic":
+                margin = -1.0 * mi
+                mult = (1.0 / (1.0 + _exp(margin))) - yi
+                li = _log1p_exp(margin) if yi > 0 else _log1p_exp(margin) - margin
+            elif kind in ("least_squares", "least_squares_half"):
+                diff = mi - yi
+                mult, li = (2.0 * diff, diff * diff) if kind == "least_squares" else (diff, diff * diff / 2.0)
+            else:
+                s = 2 * yi - 1.0
+                call = 1.0 > s * mi
+                mult, li = (-s, 1.0 - s * mi) if call else (0.0, 0.0)
+            if call and X is not None and mult != 0.0:
+                g += mult * Xd[i]
+            elif call and X is None:
+                for k in range(int(rowptr[i]), int(rowptr[i + 1])):
+                    g[idx[k]] += mult * float(val[k])
+            loss = loss + li
+            cnt += 1
+    return loss, cnt, g

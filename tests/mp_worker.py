@@ -33,6 +33,28 @@ def make_csr(n, d, k, seed):
     return np.arange(n + 1, dtype=np.int64) * k, idx, val, y
 
 
+MB_ITERS, MB_FRACTION = 6, 0.25
+
+
+def minibatch_poisoned(X, world):
+    """X with +inf, -inf and NaN in rows of rank 1 (and rank 2) that the mini-batch mask of a MB_ITERS-iteration run drops
+    in every iteration.  Loaded shards number rank r's rows from r << 40.  Returns (X, poisoned global rows)."""
+    from k1_reference import row_selected
+    X = X.copy()
+    n = X.shape[0]
+    rows = []
+    for r in range(1, world):
+        lo, hi = r * n // world, (r + 1) * n // world
+        ids = (r << 40) + np.arange(hi - lo)
+        never = np.ones(hi - lo, bool)
+        for i in range(1, MB_ITERS + 1):
+            never &= ~row_selected(42 + i, int(np.ldexp(MB_FRACTION, 64)), ids)
+        for t, i in enumerate(np.nonzero(never)[0][[0, 7, -1]]):
+            X[lo + i, 3 + t] = (np.inf, -np.inf, np.nan)[t]
+            rows.append(lo + i)
+    return X, rows
+
+
 def main():
     rank, world, port, dev, transport, out = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4]), sys.argv[5], sys.argv[6]
     import torch
@@ -77,6 +99,10 @@ def main():
     syn = ctx.synthetic(20000, 512, S.LogisticGradient(), seed=42, store="f32")
     ws, hs, ss = S.run_with_stats(syn, S.LogisticGradient(), S.SimpleUpdater(), 0.0, 5, 0.0, np.zeros(512))
     res["synthetic"] = {"w": ws.tolist(), "hist": hs.tolist(), "passes": ss.passes, "rows_local": syn.local_rows(0)}
+    # the same shard on the ring kernel with the mini-batch mask: rank r's rows start at r * n / W
+    syn.set_option("k1_variant", "ring")
+    wsm, hsm = S.GradientDescent.runMiniBatchSGD(syn, S.LogisticGradient(), S.SquaredL2Updater(), 0.5, 8, 0.01, 0.25, np.zeros(512))
+    res["minibatch_f32_ring_synthetic"] = {"w": wsm.tolist(), "hist": hsm.tolist()}
     syn.close()
     # mini-batch runs on bf16 shards through the wgmma kernel: the row mask is keyed by the global row id, so every rank
     # but 0 needs its shard's row_base.  Generated in place: rank r's rows start at r * n / W (the oracle's row ids);
@@ -94,6 +120,23 @@ def main():
     wl, hl = S.GradientDescent.runMiniBatchSGD(ldb, S.LogisticGradient(), S.SimpleUpdater(), 0.5, 6, 0.0, 0.25, np.zeros(d))
     res["minibatch_bf16_loaded"] = {"w": wl.tolist(), "hist": hl.tolist()}
     ldb.close()
+    # mini-batch runs on loaded shards of every other kernel, rows numbered from r << 40; rows of ranks >= 1 that the mask
+    # drops in every iteration hold +-inf / NaN, so the mask and the skip rule are tested together on a nonzero row_base
+    Xp, _ = minibatch_poisoned(X, world)
+    Xr = Xp[lo:hi]
+    for key, store, variant in (("f32_ring", "f32", "ring"), ("f64_generic", "f64", "generic"), ("bf16_ring", "bf16", "ring"),
+                                ("csr_f32", "f32", None), ("csr_f64", "f64", None)):
+        if variant is None:
+            Xc = Xr if store == "f32" else Xr.astype(np.float64)
+            ds = ctx.parallelize_csr(y[lo:hi], np.arange(hi - lo + 1, dtype=np.int64) * d,
+                                     np.tile(np.arange(d, dtype=np.int32), hi - lo), Xc.ravel(), d, store=store)
+        else:
+            ds = ctx.parallelize(y[lo:hi], Xr, store=store)
+            ds.set_option("k1_variant", variant)
+        wk, hk = S.GradientDescent.runMiniBatchSGD(ds, S.LogisticGradient(), S.SimpleUpdater(), 0.5, MB_ITERS, 0.0,
+                                                   MB_FRACTION, np.zeros(d))
+        res["minibatch_loaded_" + key] = {"w": wk.tolist(), "hist": hk.tolist(), "kernel": ds.kernel_name(0)}
+        ds.close()
     # a wide sparse shard: d + 4 = 100004 doubles per sweep takes the reduce-scatter + all-gather form of the exchange
     n3, d3, k3 = 9000, 100000, 12
     rp, ix, va, y3 = make_csr(n3, d3, k3, 13)
@@ -103,7 +146,7 @@ def main():
     l3, g3, c3 = wide.smooth(S.HingeGradient(), w3)
     ww, hw, sw = S.run_with_stats(wide, S.HingeGradient(), S.SquaredL2Updater(), 0.0, 5, 0.05, np.zeros(d3))
     wm3, hm3, sm3 = S.run_with_stats(wide, S.HingeGradient(), S.SquaredL2Updater(), 0.0, 5, 0.05, np.zeros(d3), memoize=True)
-    res["wide"] = {"loss": l3, "grad_l2": float(np.linalg.norm(g3)), "grad_head": g3[:64].tolist(), "count": c3,
+    res["wide"] = {"loss": l3, "grad": g3.tolist(), "count": c3,
                    "w_l2": float(np.linalg.norm(ww)), "w_head": ww[:64].tolist(), "hist": hw.tolist(), "passes": sw.passes,
                    "collective_kind": sw.collective_kind, "memo_hist": hm3.tolist(), "memo_w_l2": float(np.linalg.norm(wm3))}
     wide.close()

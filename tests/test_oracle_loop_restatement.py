@@ -15,6 +15,13 @@ def log1p_exp(x):                                   # MLUtils.log1pExp [mllib-1.
     return x + math.log1p(math.exp(-x)) if x > 0 else math.log1p(math.exp(x))
 
 
+def axpy(a, x, cum):                                # dense BLAS.axpy: netlib DAXPY, which starts with IF (DA.EQ.0) RETURN
+    if a == 0.0:
+        return
+    for j in range(len(x)):
+        cum[j] += a * x[j]
+
+
 def gradient_compute(kind, x, label, w, cum):       # Gradient.compute(data, label, weights, cumGradient): Double
     dot = 0.0
     for j in range(len(x)):
@@ -22,18 +29,15 @@ def gradient_compute(kind, x, label, w, cum):       # Gradient.compute(data, lab
     if kind == "logistic":
         margin = -1.0 * dot
         mult = (1.0 / (1.0 + math.exp(margin))) - label
-        for j in range(len(x)):
-            cum[j] += mult * x[j]
+        axpy(mult, x, cum)
         return log1p_exp(margin) if label > 0 else log1p_exp(margin) - margin
     if kind == "least_squares":
         diff = dot - label
-        for j in range(len(x)):
-            cum[j] += (2.0 * diff) * x[j]
+        axpy(2.0 * diff, x, cum)
         return diff * diff
     s = 2 * label - 1.0                             # hinge
     if 1.0 > s * dot:
-        for j in range(len(x)):
-            cum[j] += (-s) * x[j]
+        axpy(-s, x, cum)
         return 1.0 - s * dot
     return 0.0
 
