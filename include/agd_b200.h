@@ -191,6 +191,21 @@ int agd_smooth_pair(agd_handle *h, int32_t gradient, const double *w, const doub
  * at most 512 16-byte vectors per row (d <= 2048 fp32, <= 1024 fp64) and bf16 shards on the wgmma kernel; fails elsewhere. */
 int agd_smooth_two(agd_handle *h, int32_t gradient, const double *w, const double *w2, double *loss, double *grad,
                    int64_t *count, double *loss2, double *grad2);
+/* ---- scoring the resident shards (GeneralizedLinearModel.predict and model evaluation without a host copy of X) ----
+ * Both compute the margin m_i = x_i . w + b in fp64 (every element widened, products and sums by DFMA); w is d doubles.
+ * A margin depends only on the row, w, b and d: not on the row's position, the range asked for, the devices or the rank.
+ * Padded columns take zero weight, CSR margins sum exactly the row's stored entries, non-finite features follow IEEE
+ * arithmetic (an inf feature under a zero weight gives a NaN margin). */
+/* Margins of rows [row0, row0 + rows) of the shard on local device dev into out (rank-local, not collective). */
+int agd_margins(agd_handle *h, int32_t dev, const double *w, double intercept, int64_t row0, int64_t rows, double *out);
+/* The AGD_EVAL_* sums over ALL shards of the world (collective, like agd_smooth); identical bits on every rank and on
+ * every repeated call.  LOSS is the `gradient` loss of m_i (intercept included).  TP/FP/TN/FN count rows labelled exactly
+ * 0 or 1 whose predicted class is 1 when sigmoid(m) > threshold (logistic) or m > threshold (hinge); they stay 0 for the
+ * least-squares gradients.  SUM_ERR* are over e = m_i - y_i, SUM_Y* over the labels. */
+enum { AGD_EVAL_COUNT = 0, AGD_EVAL_LOSS, AGD_EVAL_TP, AGD_EVAL_FP, AGD_EVAL_TN, AGD_EVAL_FN,
+       AGD_EVAL_SUM_ERR, AGD_EVAL_SUM_ERR2, AGD_EVAL_SUM_ABS_ERR, AGD_EVAL_SUM_Y, AGD_EVAL_SUM_Y2, AGD_EVAL_N };
+int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double intercept, double threshold, double *out);
+
 /* agd_prox = applyProjector (AGD.scala:214-222): Updater.compute(w, g, step, iter = 1, reg). */
 int agd_prox(agd_handle *h, int32_t updater, const double *w, const double *g, double step, double reg,
              int32_t d, double *w_out, double *reg_val);

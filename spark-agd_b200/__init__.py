@@ -7,13 +7,15 @@ naming contract); import it as `spark_agd_b200` through the loader module at the
 """
 from . import _native
 from ._native import NativeError, build, exported_symbols
-from .glm import (GeneralizedLinearAlgorithm, LinearRegressionWithAGD, LogisticRegressionWithAGD, SVMWithAGD, append_bias,
-                  column_std)
-from .optimization import (AcceleratedGradientDescent, Context, DeviceDataset, Gradient, GradientDescent,
+from .glm import (GeneralizedLinearAlgorithm, GeneralizedLinearModel, LinearRegressionModel, LinearRegressionWithAGD,
+                  LogisticRegressionModel, LogisticRegressionWithAGD, SVMModel, SVMWithAGD, append_bias, column_std)
+from .optimization import (AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
                            HingeGradient, L1Updater, LeastSquaresGradient, LogisticGradient, MLUtils, RunStats,
                            SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, run_with_stats)
 
-__all__ = ["GeneralizedLinearAlgorithm", "LinearRegressionWithAGD", "LogisticRegressionWithAGD", "SVMWithAGD",
-           "append_bias", "column_std", "AcceleratedGradientDescent", "Context", "DeviceDataset", "Gradient", "GradientDescent",
+__all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
+           "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
+           "append_bias", "column_std", "AcceleratedGradientDescent", "Context", "DeviceDataset", "Evaluation", "Gradient",
+           "GradientDescent",
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats"]

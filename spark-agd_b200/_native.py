@@ -18,6 +18,9 @@ FLAG_MEMOIZE_FX = 1
 FLAG_NO_FUSE = 2
 ABI_VERSION = 2
 XCHG_HANDLE_BYTES = 192
+# agd_evaluate: indices of the sums it returns (AGD_EVAL_*), EVAL_N of them
+(EVAL_COUNT, EVAL_LOSS, EVAL_TP, EVAL_FP, EVAL_TN, EVAL_FN, EVAL_SUM_ERR, EVAL_SUM_ERR2, EVAL_SUM_ABS_ERR, EVAL_SUM_Y,
+ EVAL_SUM_Y2, EVAL_N) = range(12)
 
 
 class Params(C.Structure):
@@ -106,6 +109,8 @@ _SIGNATURES = {
                                   C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "agd_smooth_two": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.c_void_p,
                                  C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_void_p]),
+    "agd_margins": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p]),
+    "agd_evaluate": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
     "agd_prox": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_int32,
                            C.c_void_p, C.POINTER(C.c_double)]),
     "agd_run": (C.c_int, [C.c_void_p, C.POINTER(Params), C.c_void_p, C.c_void_p, C.c_void_p,

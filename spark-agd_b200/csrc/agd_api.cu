@@ -88,6 +88,7 @@ struct Dev {
   int32_t vec_d = 0;
   double *slabs = nullptr;
   size_t slabs_doubles = 0;
+  double *eval = nullptr;          // AGD_EVAL_N sums of agd_evaluate (this shard's, then the world's)
   double *partials = nullptr;
   unsigned int *ticket = nullptr;
   double *scalars_dev = nullptr;   // device alias of scalars_host: K3 writes its scalars straight to the host
@@ -105,7 +106,7 @@ struct Dev {
   double *hist_dev = nullptr;             // device alias of hist_host (k3_step stores the pair that rode along with a fused sweep)
   size_t hist_cap = 0;
   // K2' peer-memory exchange (xchg.cu)
-  double *xbuf = nullptr;                 // [2][W][d+4], written by every rank over NVLink
+  double *xbuf = nullptr;                 // [2][W][xchg_slot_stride(d)] (+ reduce-scatter areas), written by every rank over NVLink
   unsigned long long *xflags = nullptr;   // [2][W] epochs
   unsigned int *xticket = nullptr;
   XchgPeers xpeers;                       // every rank's xbuf / xflags as mapped into this device
@@ -360,7 +361,7 @@ int ensure_nccl(agd_handle *h) {
 // step 1 of the exchange setup: allocate this process's buffers for the current dimension and describe them
 int xchg_alloc(agd_handle *h, std::vector<XHandles> &mine) {
   const int W = h->world, nd = (int)h->devs.size();
-  const int S = 2 * (h->d + 4);              // slot stride: room for a two-gradient sweep
+  const int S = xchg_slot_stride(h->d);      // slot stride: room for a two-gradient sweep or an evaluation
   const size_t total = xchg_total_doubles(S, W), nflags = 6 * (size_t)W;   // one-shot + reduce-scatter areas (agd_common.cuh)
   mine.assign((size_t)nd, XHandles());
   for (int i = 0; i < nd; ++i) {
@@ -581,13 +582,13 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
   auto make_rs = [&](Dev &D, size_t i) {
     XchgRs x;
     x.peers = D.xpeers; x.world = h->world; x.my_rank = h->first_rank + (int)i; x.buf = (int)(epoch & 1ull);
-    x.n = n; x.slot_stride = 2 * (d + 4); x.epoch = epoch; x.ticket = D.xticket;
+    x.n = n; x.slot_stride = xchg_slot_stride(d); x.epoch = epoch; x.ticket = D.xticket;
     return x;
   };
   auto make_pub = [&](Dev &D, size_t i) {
     XchgPub pub;
     pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
-    pub.n = n; pub.slot_stride = 2 * (d + 4); pub.epoch = epoch; pub.ticket = D.xticket;
+    pub.n = n; pub.slot_stride = xchg_slot_stride(d); pub.epoch = epoch; pub.ticket = D.xticket;
     return pub;
   };
   for (size_t i = 0; i < h->devs.size(); ++i) {
@@ -665,8 +666,8 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
     for (Dev &D : h->devs) {
       CK(cudaSetDevice(D.ordinal));
-      if (rs) CK(xchg_rs_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, 2 * (d + 4), epoch, D.acc, D.st));
-      else CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, 2 * (d + 4), epoch, D.acc, D.st));
+      if (rs) CK(xchg_rs_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.acc, D.st));
+      else CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.acc, D.st));
     }
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
     trace_mark(h, "gather");
@@ -863,7 +864,7 @@ int agd_destroy(agd_handle *h) {
     if (D.comm && nccl_api().ok) nccl_api().CommDestroy(D.comm);
     D.comm = nullptr;
     free_shard(h, D);
-    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials};
+    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval};
     for (double *p : v)
       if (p) cudaFree(p);
     if (D.ticket) cudaFree(D.ticket);
@@ -1355,6 +1356,100 @@ int agd_smooth_two(agd_handle *h, int32_t gradient, const double *w, const doubl
   return smooth_host(h, gradient, w, w2, loss, grad, count, loss2, grad2);
 }
 
+// ---------------------------------------------------------------- scoring (score.cu)
+// w (d_user doubles) -> D.wtmp, zero on the padded columns
+static int stage_weights(agd_handle *h, Dev &D, const double *w) {
+  CK(cudaMemsetAsync(D.wtmp, 0, ((size_t)h->d + 2) * sizeof(double), D.st));
+  CK(cudaMemcpyAsync(D.wtmp, w, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  return 0;
+}
+
+static ScoreArgs score_args(const agd_handle *h, const Dev &D, double intercept) {
+  const Shard &s = D.sh;
+  ScoreArgs a;
+  if (s.csr) { a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; }
+  else a.X = s.X;
+  a.labels = s.labels; a.w = D.wtmp; a.b = intercept; a.d = h->d; a.stream = D.st;
+  return a;
+}
+
+int agd_margins(agd_handle *h, int32_t dev, const double *w, double intercept, int64_t row0, int64_t rows, double *out) {
+  if (!h) return 1;
+  if (dev < 0 || dev >= (int)h->devs.size()) return fail(h, "bad local device index %d", dev);
+  if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
+  Dev &D = h->devs[dev];
+  const Shard &s = D.sh;
+  if (row0 < 0 || rows < 0 || rows > s.rows - row0)
+    return fail(h, "row range [%lld, %lld + %lld) lies outside the %lld rows of device %d", (long long)row0, (long long)row0,
+                (long long)rows, (long long)s.rows, dev);
+  if (!w || (rows > 0 && !out)) return fail(h, "NULL argument");
+  if (rows == 0) return 0;
+  if (ensure_vectors(h, D, h->d)) return 1;
+  CK(cudaSetDevice(D.ordinal));
+  if (stage_weights(h, D, w)) return 1;
+  // margins depend on the row only, so the range is scored in chunks through the staging buffer
+  const int64_t chunk = rows < (int64_t)(1 << 22) ? rows : (int64_t)(1 << 22);
+  if (ensure_stage(h, D, (size_t)chunk * sizeof(double))) return 1;
+  ScoreArgs a = score_args(h, D, intercept);
+  a.margins = (double *)D.stage_dev;
+  for (int64_t r0 = 0; r0 < rows; r0 += chunk) {
+    a.row0 = row0 + r0;
+    a.rows = rows - r0 < chunk ? rows - r0 : chunk;
+    CK(score_margins_launch(a, s.elem_bytes, D.sm_count));
+    CK(cudaMemcpyAsync(out + r0, D.stage_dev, (size_t)a.rows * sizeof(double), cudaMemcpyDeviceToHost, D.st));
+    CK(cudaStreamSynchronize(D.st));   // the staging buffer is reused
+  }
+  return 0;
+}
+
+// Collective: one evaluation sweep per local shard, the fixed-order slab reduce, and the same exchange a sweep of agd_smooth
+// uses (one epoch of the peer-memory exchange with an AGD_EVAL_N-double payload, or an NCCL all-reduce).
+int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double intercept, double threshold, double *out) {
+  if (check_ready(h)) return 1;
+  if (gradient < 0 || gradient > AGD_GRAD_LEAST_SQUARES_HALF) return fail(h, "unknown gradient %d", gradient);
+  if (!w || !out) return fail(h, "NULL argument");
+  h->xg_pending = false;
+  const int32_t d = h->d, n = AGD_EVAL_N;
+  const bool p2p = h->world > 1 && h->x_p2p;
+  const unsigned long long epoch = p2p ? ++h->x_epoch : 0ull;
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    if (!D.eval) CK(cudaMalloc(&D.eval, (size_t)n * sizeof(double)));
+    if (ensure_slabs(h, D, score_max_blocks(D.sm_count), n)) return 1;
+    if (stage_weights(h, D, w)) return 1;
+    ScoreArgs a = score_args(h, D, intercept);
+    a.rows = D.sh.rows; a.kind = gradient; a.threshold = threshold; a.slabs = D.slabs;
+    int blocks = 0;
+    CK(score_eval_launch(a, D.sh.elem_bytes, D.sm_count, &blocks));
+    if (p2p) {
+      XchgPub pub;
+      pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
+      pub.n = n; pub.slot_stride = xchg_slot_stride(d); pub.epoch = epoch; pub.ticket = D.xticket;
+      CK(k1_reduce_launch(D.slabs, blocks, n, D.eval, &pub, D.st));
+    } else {
+      CK(k1_reduce_launch(D.slabs, blocks, n, D.eval, nullptr, D.st));
+    }
+  }
+  if (p2p) {
+    for (Dev &D : h->devs) {
+      CK(cudaSetDevice(D.ordinal));
+      CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.eval, D.st));
+    }
+  } else if (h->world > 1) {
+    if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
+    NcclApi &N = nccl_api();
+    CKN(N.GroupStart());
+    for (Dev &D : h->devs) CKN(N.AllReduce(D.eval, D.eval, (size_t)n, ncclDouble, ncclSum, D.comm, D.st));
+    CKN(N.GroupEnd());
+  }
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  CK(cudaMemcpyAsync(out, D0.eval, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  return 0;
+}
+
 // ---------------------------------------------------------------- applyProjector with host buffers
 int agd_prox(agd_handle *h, int32_t updater, const double *w, const double *g, double step, double reg,
              int32_t d, double *w_out, double *reg_val) {
@@ -1454,7 +1549,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
   auto take_gather = [&](Dev &D) {
     XchgGather g;
     if (h->xg_pending) {
-      const int S = 2 * (d + 4), W = h->world;
+      const int S = xchg_slot_stride(d), W = h->world;
       g.world = W; g.buf = (int)(h->xg_epoch & 1ull); g.n = h->xg_n; g.slot_stride = S; g.epoch = h->xg_epoch;
       g.rs = h->xg_rs ? 1 : 0;
       g.xbuf = h->xg_rs ? D.xbuf + xchg_off_res(S, W) : D.xbuf;       // rs: the area of finished sums

@@ -54,8 +54,9 @@ struct XchgPeers {
 struct XchgPub {
   XchgPeers peers;
   int world, my_rank, buf, n;
-  int slot_stride;          // doubles between two ranks' slots (the buffers' capacity per slot, NOT this sweep's n: sweeps of
-                            // different payloads -- d + 4 or 2 (d + 4) -- must not move the slots of the other parity buffer)
+  int slot_stride;          // doubles between two ranks' slots: xchg_slot_stride(d), the buffers' capacity per slot, NOT this
+                            // sweep's n: sweeps of different payloads -- d + 4, 2 (d + 4) or AGD_EVAL_N -- must not move the
+                            // slots of the other parity buffer
   unsigned long long epoch;
   unsigned int *ticket;
 };
@@ -72,7 +73,7 @@ struct XchgGather {
 // ---- large payloads (n >= kXchgRsMin doubles, e.g. d = 10^6): reduce-scatter + all-gather over the same peer memory.
 // Rank r stores slice p of its partial sums into rank p's `rs` area (slot r), rank p adds the W slots of ITS slice in rank order
 // and stores the finished slice into every rank's `res` area; 2 n / W doubles leave each rank per sweep instead of n W.
-// Layout of one device's exchange allocation (doubles): [one-shot: 2 W S][rs: 2 W L][res: 2 S], S = 2 (d + 4), L = ceil(S / W);
+// Layout of one device's exchange allocation (doubles): [one-shot: 2 W S][rs: 2 W L][res: 2 S], S = xchg_slot_stride(d) (below), L = ceil(S / W);
 // flags (u64): [one-shot 2 W][rs arrived 2 W][res arrived 2 W].
 constexpr int kXchgRsMin = 32768;
 struct XchgRs {
@@ -117,6 +118,35 @@ struct K1CsrArgs {
   int32_t tune;           // option ring_rows: 1 = the simple (unpipelined) loop
 };
 cudaError_t k1_csr_launch(const K1CsrArgs &a, int elem_bytes, int sm_count, cudaStream_t st);
+
+// Slot stride of the peer-memory exchange (doubles per rank's slot): the largest payload any sweep on a handle of this
+// dimension publishes -- 2 (d + 4) for a two-gradient sweep, AGD_EVAL_N for an evaluation.  ONE stride per handle: sweeps
+// of different payloads must not move the slots of the other parity buffer.
+inline int xchg_slot_stride(int32_t d) { return 2 * (d + 4) > AGD_EVAL_N ? 2 * (d + 4) : AGD_EVAL_N; }
+
+// ---------------------------------------------------------------- scoring sweeps (score.cu)
+// Margins m_i = x_i . w + b of rows [row0, row0 + rows) of one shard, or the AGD_EVAL_* sums over them (one slab of
+// AGD_EVAL_N doubles per CTA, added in fixed order by k1_reduce_launch).  Dense (rowptr == nullptr) or CSR.
+struct ScoreArgs {
+  const void *X = nullptr;          // dense shard, row-major, ld == d (fp32 / fp64 / bf16)
+  const int64_t *rowptr = nullptr;  // CSR shard (fp32 / fp64 values)
+  const int32_t *idx = nullptr;
+  const void *val = nullptr;
+  const double *labels = nullptr;
+  const double *w = nullptr;        // d doubles (device), zero on padded columns
+  double b = 0.0;                   // intercept
+  int64_t row0 = 0, rows = 0;
+  int32_t d = 0;                    // stored row length (the handle's internal dimension)
+  int32_t kind = 0;                 // AGD_GRAD_* (evaluation)
+  double threshold = 0.0;           // evaluation: confusion-count threshold
+  double *margins = nullptr;        // margins form: rows doubles
+  double *slabs = nullptr;          // evaluation form: [score_max_blocks][AGD_EVAL_N]
+  cudaStream_t stream = nullptr;
+};
+int score_max_blocks(int sm_count);
+cudaError_t score_margins_launch(const ScoreArgs &a, int elem_bytes, int sm_count);
+// *blocks_out = slabs written (0 for an empty range)
+cudaError_t score_eval_launch(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out);
 
 
 // ---------------------------------------------------------------- K3: fused O(d) driver-side vector work

@@ -15,35 +15,82 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .optimization import (AcceleratedGradientDescent, Context, HingeGradient, LeastSquaresGradient, LogisticGradient,
-                           SimpleUpdater, SquaredL2Updater)
+from .optimization import (AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, HingeGradient,
+                           LeastSquaresGradient, LogisticGradient, SimpleUpdater, SquaredL2Updater)
 
 
 @dataclass
 class GeneralizedLinearModel:
     weights: np.ndarray
     intercept: float
+    loss = None    # the Gradient whose loss evaluate() reports; the concrete models below name theirs
 
     def margin(self, X) -> np.ndarray:
+        """x . weights + intercept per row; X is a host matrix or a DeviceDataset (scored where it is resident)."""
+        if isinstance(X, DeviceDataset):
+            return X.margins(self.weights, self.intercept)
         return np.asarray(X, dtype=np.float64) @ self.weights + self.intercept
 
+    def evaluate(self, data: DeviceDataset) -> Evaluation:
+        """The model's loss, confusion counts (at its threshold) and error moments over every shard of `data`'s world
+        (collective)."""
+        if self.loss is None:
+            raise TypeError(f"{type(self).__name__} names no loss: evaluate() needs a model class with a `loss` Gradient "
+                            "(LogisticRegressionModel, SVMModel, LinearRegressionModel)")
+        return data.evaluate(self.loss, self.weights, self.intercept, self._eval_threshold())
 
-class LogisticRegressionModel(GeneralizedLinearModel):
-    threshold = 0.5
+    def _eval_threshold(self) -> float:
+        return 0.5
+
+
+class _ThresholdModel(GeneralizedLinearModel):
+    """setThreshold / clearThreshold of the binary classification models (mllib 1.3.0): with the threshold cleared,
+    predict returns the raw score.  Until set, the class default applies."""
+
+    def setThreshold(self, threshold: float):
+        self.threshold = float(threshold)
+        return self
+
+    def clearThreshold(self):
+        self.threshold = None
+        return self
+
+    def getThreshold(self):
+        return self.threshold
+
+    def score(self, X) -> np.ndarray:
+        raise NotImplementedError
 
     def predict(self, X) -> np.ndarray:
-        score = 1.0 / (1.0 + np.exp(-self.margin(X)))
+        score = self.score(X)
+        if self.threshold is None:
+            return score
         return (score > self.threshold).astype(np.float64)
 
+    def _eval_threshold(self) -> float:
+        # the confusion counts need a cut even when predict returns raw scores: the class default then
+        return type(self).threshold if self.threshold is None else self.threshold
 
-class SVMModel(GeneralizedLinearModel):
+
+class LogisticRegressionModel(_ThresholdModel):
+    threshold = 0.5
+    loss = LogisticGradient()
+
+    def score(self, X) -> np.ndarray:
+        return 1.0 / (1.0 + np.exp(-self.margin(X)))
+
+
+class SVMModel(_ThresholdModel):
     threshold = 0.0
+    loss = HingeGradient()
 
-    def predict(self, X) -> np.ndarray:
-        return (self.margin(X) > self.threshold).astype(np.float64)
+    def score(self, X) -> np.ndarray:
+        return self.margin(X)
 
 
 class LinearRegressionModel(GeneralizedLinearModel):
+    loss = LeastSquaresGradient()
+
     def predict(self, X) -> np.ndarray:
         return self.margin(X)
 
@@ -95,7 +142,19 @@ class GeneralizedLinearAlgorithm:
             X = append_bias(X)
         return X, scale
 
-    def run(self, sc: Context, labels, X, initialWeights=None):
+    def run(self, sc, *args, **kwargs):
+        """Two forms:
+          run(sc, labels, X, initialWeights=None)  pins the transformed host rows on the context's GPUs and trains on them;
+          run(data, initialWeights=None)           trains on a DeviceDataset where it is resident (e.g. MLUtils.loadLibSVMFile).
+        The second form takes nothing but the initial weights (positionally or by that name)."""
+        if isinstance(sc, DeviceDataset):
+            if len(args) + len(kwargs) > 1 or set(kwargs) - {"initialWeights"}:
+                raise TypeError("run(data[, initialWeights]): a DeviceDataset already holds the labels and the rows; "
+                                "only the initial weights may follow it")
+            return self._run_resident(sc, *args, **kwargs)
+        return self._run_host(sc, *args, **kwargs)
+
+    def _run_host(self, sc: Context, labels, X, initialWeights=None):
         Xt, scale = self.prepare(X)
         d = np.asarray(X).shape[1]
         # GeneralizedLinearAlgorithm.run [mllib-1.3.0]: initialWeights default to zeros(numFeatures), and with addIntercept
@@ -115,6 +174,21 @@ class GeneralizedLinearAlgorithm:
         if self.useFeatureScaling:
             weights = weights * scale          # back to the original feature scale
         return self.model_class(weights, intercept)
+
+    def _run_resident(self, data: DeviceDataset, initialWeights=None):
+        # both switches rewrite every row (appendBias / StandardScaler); the resident shard is used as it is
+        if self.addIntercept:
+            raise ValueError("run(DeviceDataset) cannot add an intercept: it needs a copy of the resident shard with a "
+                             "column of ones appended; train from host rows (run(sc, labels, X)) instead")
+        if self.useFeatureScaling:
+            raise ValueError("run(DeviceDataset) cannot scale features: it needs a rescaled copy of the resident shard; "
+                             "train from host rows (run(sc, labels, X)) instead")
+        d = data.d
+        w0 = np.zeros(d) if initialWeights is None else np.asarray(initialWeights, dtype=np.float64)
+        if w0.ndim != 1 or w0.shape[0] != d:
+            raise ValueError(f"initialWeights has size {w0.shape}, data has {d} features")
+        w = self.optimizer.optimize(data, w0)
+        return self.model_class(np.array(w, dtype=np.float64), 0.0)
 
 
 class LogisticRegressionWithAGD(GeneralizedLinearAlgorithm):

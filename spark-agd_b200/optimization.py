@@ -334,6 +334,35 @@ class DeviceDataset:
                                        C.byref(cnt), C.byref(loss2), _ptr(g2)), self.h)
         return loss.value, g, cnt.value, loss2.value, g2
 
+    # scoring the resident shards (no host copy of X)
+    def _weights(self, w) -> np.ndarray:
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        if w.ndim != 1 or w.shape[0] != self.d:
+            raise ValueError(f"weights have size {w.shape}, data has {self.d} features")
+        return w
+
+    def margins_rows(self, dev: int, row0: int, rows: int, w, intercept: float = 0.0) -> np.ndarray:
+        """x_i . w + intercept (fp64) of rows [row0, row0 + rows) of local device `dev`'s shard (not collective)."""
+        w = self._weights(w)
+        out = np.empty(max(int(rows), 0), dtype=np.float64)
+        N.check(N.lib().agd_margins(self.h, dev, _ptr(w), float(intercept), int(row0), int(rows), _ptr(out)), self.h)
+        return out
+
+    def margins(self, w, intercept: float = 0.0) -> np.ndarray:
+        """x_i . w + intercept (fp64) of this process's rows, across its local devices in load order (not collective)."""
+        return np.concatenate([self.margins_rows(i, 0, self.local_rows(i), w, intercept)
+                               for i in range(len(self.ctx.devices))])
+
+    def evaluate(self, gradient: Gradient, w, intercept: float = 0.0, threshold: float = 0.5) -> "Evaluation":
+        """Loss, confusion counts and error moments of the model (w, intercept) over every shard of the world, from one
+        read of X (collective: every rank calls it; every rank gets the same bits)."""
+        w = self._weights(w)
+        sums = np.empty(N.EVAL_N, dtype=np.float64)
+        self._ensure_exchange()
+        N.check(N.lib().agd_evaluate(self.h, _grad_kind(gradient), _ptr(w), float(intercept), float(threshold), _ptr(sums)),
+                self.h)
+        return Evaluation.from_sums(sums)
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
@@ -389,6 +418,65 @@ class MLUtils:
         N.check(N.lib().agd_load_libsvm(ds.h, path.encode(), numFeatures, _STORE[store]), ds.h)
         ds.total_rows = sum(ds.local_rows(i) for i in range(len(sc.devices)))
         return ds
+
+
+def _ratio(a: float, b: float) -> float:
+    return a / b if b != 0 else float("nan")
+
+
+@dataclass(frozen=True)
+class Evaluation:
+    """The sums agd_evaluate reduces over the world (AGD_EVAL_*), and the metrics derived from them on the host.
+    Confusion counts cover rows labelled exactly 0 or 1 under the logistic / hinge losses; e = margin - label."""
+    count: float
+    loss_sum: float
+    tp: float
+    fp: float
+    tn: float
+    fn: float
+    sum_err: float
+    sum_err2: float
+    sum_abs_err: float
+    sum_y: float
+    sum_y2: float
+
+    @classmethod
+    def from_sums(cls, sums) -> "Evaluation":
+        return cls(*(float(v) for v in np.asarray(sums, dtype=np.float64)[:N.EVAL_N]))
+
+    @property
+    def mean_loss(self) -> float:
+        """loss_sum / count: the loss applySmooth reports (AGD.scala:207), with the intercept inside the margin."""
+        return _ratio(self.loss_sum, self.count)
+
+    @property
+    def accuracy(self) -> float:
+        return _ratio(self.tp + self.tn, self.tp + self.fp + self.tn + self.fn)
+
+    @property
+    def precision(self) -> float:
+        return _ratio(self.tp, self.tp + self.fp)
+
+    @property
+    def recall(self) -> float:
+        return _ratio(self.tp, self.tp + self.fn)
+
+    @property
+    def mse(self) -> float:
+        return _ratio(self.sum_err2, self.count)
+
+    @property
+    def rmse(self) -> float:
+        return float(np.sqrt(self.mse))
+
+    @property
+    def mae(self) -> float:
+        return _ratio(self.sum_abs_err, self.count)
+
+    @property
+    def r2(self) -> float:
+        """1 - SSE / (sum y^2 - (sum y)^2 / n)."""
+        return 1.0 - _ratio(self.sum_err2, self.sum_y2 - _ratio(self.sum_y ** 2, self.count))
 
 
 @dataclass
