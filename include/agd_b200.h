@@ -206,6 +206,23 @@ enum { AGD_EVAL_COUNT = 0, AGD_EVAL_LOSS, AGD_EVAL_TP, AGD_EVAL_FP, AGD_EVAL_TN,
        AGD_EVAL_SUM_ERR, AGD_EVAL_SUM_ERR2, AGD_EVAL_SUM_ABS_ERR, AGD_EVAL_SUM_Y, AGD_EVAL_SUM_Y2, AGD_EVAL_N };
 int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double intercept, double threshold, double *out);
 
+/* ---- views of the resident shards (RDD.randomSplit / sample / MLUtils.kFold without copying a row) ----
+ * Every row has a 64-bit draw u = Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, 7), words 0 and 1, where grow
+ * = the shard's first global row + local row (the numbering of the mini-batch mask: a generated shard's global row, or
+ * rank << 40 + row on loaded shards, so views of loaded shards depend on the partitioning).  Predicate i holds iff
+ * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
+ * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
+ * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
+ * mask) and agd_evaluate, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
+ * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
+ * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */
+int agd_set_row_filter(agd_handle *h, int32_t n, const uint64_t *seeds, const double *lo, const double *hi,
+                       const int32_t *complement);
+/* out[i] = 1 if physical row row0 + i of the shard on local device dev is in the current view, else 0 (rank-local, not
+ * collective; the kernels' own predicate, so a host never restates the draw). */
+int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, uint8_t *out);
+
 /* agd_prox = applyProjector (AGD.scala:214-222): Updater.compute(w, g, step, iter = 1, reg). */
 int agd_prox(agd_handle *h, int32_t updater, const double *w, const double *g, double step, double reg,
              int32_t d, double *w_out, double *reg_val);

@@ -9,13 +9,14 @@ from . import _native
 from ._native import NativeError, build, exported_symbols
 from .glm import (GeneralizedLinearAlgorithm, GeneralizedLinearModel, LinearRegressionModel, LinearRegressionWithAGD,
                   LogisticRegressionModel, LogisticRegressionWithAGD, SVMModel, SVMWithAGD, append_bias, column_std)
-from .optimization import (AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
+from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
                            HingeGradient, L1Updater, LeastSquaresGradient, LogisticGradient, MLUtils, RunStats,
-                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, run_with_stats)
+                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, run_with_stats, split_bounds)
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
            "append_bias", "column_std", "AcceleratedGradientDescent", "Context", "DeviceDataset", "Evaluation", "Gradient",
            "GradientDescent",
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
-           "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats"]
+           "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
+           "DEFAULT_SPLIT_SEED", "split_bounds"]

@@ -111,6 +111,8 @@ _SIGNATURES = {
                                  C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_void_p]),
     "agd_margins": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_evaluate": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
+    "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "agd_row_filter_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_prox": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_int32,
                            C.c_void_p, C.POINTER(C.c_double)]),
     "agd_run": (C.c_int, [C.c_void_p, C.POINTER(Params), C.c_void_p, C.c_void_p, C.c_void_p,

@@ -102,6 +102,12 @@ struct Dev {
   size_t ev_ar_used = 0;
   std::mutex *mu = nullptr;
   long long row_base = 0;          // global index of this shard's first row (for the sampling mask)
+  RowFilter *filt_dev = nullptr;   // device copy of the handle's row filter (agd_set_row_filter)
+  uint32_t *view_bits = nullptr;   // the filter as a bitmap of this shard's rows (the ring kernel reads it), see ensure_view_bits
+  size_t view_bits_words = 0;      // capacity
+  int64_t view_bits_rows = -1;     // rows the bitmap describes (-1: none) ...
+  long long view_bits_base = 0;    // ... numbered from this row_base ...
+  RowFilter view_bits_filt;        // ... under this filter
   double *hist_host = nullptr;            // pinned + mapped: [2k] = loss sum, [2k+1] = count of the history pass of iteration k
   double *hist_dev = nullptr;             // device alias of hist_host (k3_step stores the pair that rode along with a fused sweep)
   size_t hist_cap = 0;
@@ -129,6 +135,8 @@ struct agd_handle {
   int k1_diag = 0;
   int tc_margins_f64 = 0;    // wgmma kernel: fp64-exact margins instead of the fp32 phase 1
   unsigned long long sample_seed = 0, sample_thresh = 0;  // mini-batch row mask of the current pass (0 = every row)
+  RowFilter filt;            // the view every collective sweep runs on (agd_set_row_filter; n = 0: every row) ...
+  const RowFilter *filt_of(const Dev &D) const { return filt.n ? D.filt_dev : nullptr; }   // ... as the kernels get it
   int collective = 0;        // 0 = auto (peer memory if every pair of ranks can map each other, else NCCL), 1 = nccl, 2 = p2p
   int32_t x_d = 0;           // dimension the exchange buffers were built for (0 = not built)
   bool x_p2p = false;        // exchange buffers are live
@@ -294,6 +302,34 @@ int ensure_stage(agd_handle *h, Dev &D, size_t bytes) {
   D.stage_dev = nullptr;
   CK(cudaMalloc(&D.stage_dev, bytes));
   D.stage_bytes = bytes;
+  return 0;
+}
+
+// The current filter as a bitmap of D's rows, drawn by the kernels' own row_in_view() (one launch, one Philox per row and
+// predicate): rebuilt when the filter, the shard's row count or its row numbering changed since the last build, so a run of
+// many sweeps on one view draws its rows once.  One bit per row (rows / 8 bytes next to the shard).
+int ensure_view_bits(agd_handle *h, Dev &D) {
+  if (h->filt.n == 0) return 0;
+  const int64_t rows = D.sh.rows;
+  const RowFilter &f = h->filt;
+  bool same = D.view_bits_rows == rows && D.view_bits_base == D.row_base && D.view_bits_filt.n == f.n;
+  for (int i = 0; same && i < f.n; ++i)
+    same = D.view_bits_filt.seed[i] == f.seed[i] && D.view_bits_filt.lo[i] == f.lo[i] && D.view_bits_filt.hi[i] == f.hi[i] &&
+           D.view_bits_filt.flags[i] == f.flags[i];
+  if (same) return 0;
+  const size_t words = (size_t)((rows + 31) / 32) + 1;
+  if (D.view_bits_words < words) {
+    if (D.view_bits) cudaFree(D.view_bits);
+    D.view_bits = nullptr;
+    D.view_bits_words = 0;
+    CK(cudaMalloc(&D.view_bits, words * sizeof(uint32_t)));
+    D.view_bits_words = words;
+  }
+  CK(row_filter_bits_launch(D.filt_dev, D.row_base, rows, D.view_bits, D.st));
+  if (&D == &h->devs[0]) h->launches += 1;
+  D.view_bits_rows = rows;
+  D.view_bits_base = D.row_base;
+  D.view_bits_filt = f;
   return 0;
 }
 
@@ -602,7 +638,7 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
       a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; a.labels = s.labels; a.w = w_of(D);
       a.w2 = w2_of ? w2_of(D) : nullptr;
       a.gacc = D.acc; a.rows = s.rows; a.d = d; a.kind = kind;
-      a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.tune = h->tune_rows;
+      a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.filt = h->filt_of(D); a.tune = h->tune_rows;
       if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
       CK(k1_csr_launch(a, s.elem_bytes, D.sm_count, D.st));
       if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
@@ -614,11 +650,12 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
       h->launches += (i == 0) ? (rs ? 4 : (p2p ? 3 : 2)) : 0;
       continue;
     }
+    if (ensure_view_bits(h, D)) return 1;
     K1Args a;
     a.X = s.X; a.labels = s.labels; a.w = w_of(D); a.w2 = w2_of ? w2_of(D) : nullptr; a.dual_full = dual_full ? 1 : 0;
     a.rows = s.rows; a.d = d; a.kind = h->k1_diag ? h->k1_diag : kind;
     a.stages = h->ring_stages; a.slab_stride = n;
-    a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.tune_rows = h->tune_rows; a.tune_ctas = h->tune_ctas; a.tune_full = h->tune_full;
+    a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.filt = h->filt_of(D); a.view_bits = a.filt ? D.view_bits : nullptr; a.tune_rows = h->tune_rows; a.tune_ctas = h->tune_ctas; a.tune_full = h->tune_full;
     a.tc_margins_f64 = h->tc_margins_f64;
     const int eb = s.elem_bytes ? s.elem_bytes : 4;
     bool ring = k1_ring_supported(d, eb) != 0;
@@ -871,6 +908,8 @@ int agd_destroy(agd_handle *h) {
     if (D.scalars_host) cudaFreeHost(D.scalars_host);
     if (D.hist_host) cudaFreeHost(D.hist_host);
     if (D.stage_dev) cudaFree(D.stage_dev);
+    if (D.filt_dev) cudaFree(D.filt_dev);
+    if (D.view_bits) cudaFree(D.view_bits);
     for (cudaEvent_t e : D.ev) cudaEventDestroy(e);
     for (cudaEvent_t e : D.ev_ar) cudaEventDestroy(e);
     if (&D == &h->devs[0] && h->ev_begin) { cudaEventDestroy(h->ev_begin); cudaEventDestroy(h->ev_end); }
@@ -1189,6 +1228,7 @@ int agd_clear(agd_handle *h) {
   }
   h->d = 0;
   h->d_user = 0;
+  h->filt = RowFilter();
   return 0;
 }
 
@@ -1420,6 +1460,7 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
     if (stage_weights(h, D, w)) return 1;
     ScoreArgs a = score_args(h, D, intercept);
     a.rows = D.sh.rows; a.kind = gradient; a.threshold = threshold; a.slabs = D.slabs;
+    a.row_base = D.row_base; a.filt = h->filt_of(D);
     int blocks = 0;
     CK(score_eval_launch(a, D.sh.elem_bytes, D.sm_count, &blocks));
     if (p2p) {
@@ -1447,6 +1488,62 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
   CK(cudaSetDevice(D0.ordinal));
   CK(cudaMemcpyAsync(out, D0.eval, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
   for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  return 0;
+}
+
+// ---------------------------------------------------------------- views (row filters)
+int agd_set_row_filter(agd_handle *h, int32_t n, const uint64_t *seeds, const double *lo, const double *hi,
+                       const int32_t *complement) {
+  if (!h) return 1;
+  if (n < 0 || n > kMaxRowPredicates) return fail(h, "a row filter holds 0 to %d predicates (got %d)", kMaxRowPredicates, n);
+  if (n > 0 && (!seeds || !lo || !hi || !complement)) return fail(h, "NULL argument");
+  RowFilter f;
+  f.n = n;
+  for (int i = 0; i < n; ++i) {
+    if (!(lo[i] >= 0.0 && lo[i] <= hi[i] && hi[i] <= 1.0))   // also refuses NaN
+      return fail(h, "predicate %d: bounds must satisfy 0 <= lo <= hi <= 1 (lo=%.17g, hi=%.17g)", i, lo[i], hi[i]);
+    if (complement[i] != 0 && complement[i] != 1) return fail(h, "predicate %d: complement must be 0 or 1 (got %d)", i, complement[i]);
+    // b = floor(c 2^64): exact for c < 1 (ldexp is exact and the result is below 2^64); c = 1 is "to the end"
+    f.seed[i] = seeds[i];
+    f.lo[i] = lo[i] < 1.0 ? (unsigned long long)std::ldexp(lo[i], 64) : 0ull;
+    f.hi[i] = hi[i] < 1.0 ? (unsigned long long)std::ldexp(hi[i], 64) : 0ull;
+    f.flags[i] = (complement[i] ? kRowPredComplement : 0u) | (lo[i] < 1.0 ? 0u : kRowPredLoEnd) | (hi[i] < 1.0 ? 0u : kRowPredHiEnd);
+  }
+  // Until every device holds the new filter the handle runs without one: a failure part-way leaves no device on a filter the
+  // handle does not describe (the call then fails and the handle has no filter).
+  h->filt = RowFilter();
+  auto upload = [&]() -> int {
+    for (Dev &D : h->devs) {   // stream-ordered after every sweep that still reads the previous filter
+      CK(cudaSetDevice(D.ordinal));
+      if (!D.filt_dev) CK(cudaMalloc(&D.filt_dev, sizeof(RowFilter)));
+      CK(cudaMemcpyAsync(D.filt_dev, &f, sizeof(RowFilter), cudaMemcpyHostToDevice, D.st));
+      CK(cudaStreamSynchronize(D.st));
+    }
+    return 0;
+  };
+  if (upload()) return 1;
+  h->filt = f;
+  return 0;
+}
+
+int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, uint8_t *out) {
+  if (!h) return 1;
+  if (dev < 0 || dev >= (int)h->devs.size()) return fail(h, "bad local device index %d", dev);
+  Dev &D = h->devs[dev];
+  if (row0 < 0 || rows < 0 || rows > D.sh.rows - row0)
+    return fail(h, "row range [%lld, %lld + %lld) lies outside the %lld rows of device %d", (long long)row0, (long long)row0,
+                (long long)rows, (long long)D.sh.rows, dev);
+  if (rows > 0 && !out) return fail(h, "NULL argument");
+  if (rows == 0) return 0;
+  CK(cudaSetDevice(D.ordinal));
+  const int64_t chunk = rows < (int64_t)(1 << 24) ? rows : (int64_t)(1 << 24);
+  if (ensure_stage(h, D, (size_t)chunk)) return 1;
+  for (int64_t r0 = 0; r0 < rows; r0 += chunk) {
+    const int64_t m = rows - r0 < chunk ? rows - r0 : chunk;
+    CK(row_filter_mask_launch(h->filt_of(D), D.row_base + row0 + r0, m, (uint8_t *)D.stage_dev, D.st));
+    CK(cudaMemcpyAsync(out + r0, D.stage_dev, (size_t)m, cudaMemcpyDeviceToHost, D.st));
+    CK(cudaStreamSynchronize(D.st));   // the staging buffer is reused
+  }
   return 0;
 }
 

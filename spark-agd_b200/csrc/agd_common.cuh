@@ -7,6 +7,19 @@
 
 namespace agd {
 
+// ---------------------------------------------------------------- views of the resident shards (agd_set_row_filter)
+// A conjunction of up to kMaxRowPredicates predicates on the row's own 64-bit draw u(seed, grow) (row_in_view(),
+// k1_device.cuh).  Predicate i holds iff lo_i <= u < hi_i, negated under kRowPredComplement; a bound of exactly 2^64 (c = 1)
+// is carried as a flag, since it does not fit the integer.  The kernels read it from device memory through a pointer in their
+// arguments; a null pointer means every row, and they test that first, uniformly.
+constexpr int kMaxRowPredicates = 4;
+enum { kRowPredComplement = 1, kRowPredLoEnd = 2, kRowPredHiEnd = 4 };
+struct RowFilter {
+  int32_t n = 0;
+  uint32_t flags[kMaxRowPredicates] = {};
+  unsigned long long seed[kMaxRowPredicates] = {}, lo[kMaxRowPredicates] = {}, hi[kMaxRowPredicates] = {};
+};
+
 // ---------------------------------------------------------------- K1: fused row-block gradient
 // Replaces the seqOp fold of AGD.scala:197-200 + Gradient.compute [mllib-1.3.0] over one shard.
 struct K1Args {
@@ -23,6 +36,9 @@ struct K1Args {
   int32_t slab_stride;    // d + 4
   unsigned long long sample_seed, sample_thresh;  // Bernoulli row mask (thresh 0 = every row), see row_selected()
   long long row_base;     // global index of the shard's first row
+  const RowFilter *filt;  // the view a collective call runs on (device copy; nullptr: every row), see row_in_view()
+  const uint32_t *view_bits;  // with filt: bit r % 32 of word r / 32 = row_in_view() of local row r, drawn when the filter
+                              // was set (the ring and wgmma kernels read these: no Philox between their barriers)
   int32_t tune_rows;      // 0 = default; rows per tile of the headline ring shape (4|8)
   int32_t tune_ctas;      // 0 = default; resident CTAs per SM (1|2|3)
   int32_t tune_full;      // 0 = default; 1 = keep the column predicates even when every thread owns whole vectors
@@ -115,6 +131,7 @@ struct K1CsrArgs {
   int32_t kind;
   unsigned long long sample_seed, sample_thresh;
   long long row_base;
+  const RowFilter *filt;  // as in K1Args
   int32_t tune;           // option ring_rows: 1 = the simple (unpipelined) loop
 };
 cudaError_t k1_csr_launch(const K1CsrArgs &a, int elem_bytes, int sm_count, cudaStream_t st);
@@ -141,12 +158,18 @@ struct ScoreArgs {
   double threshold = 0.0;           // evaluation: confusion-count threshold
   double *margins = nullptr;        // margins form: rows doubles
   double *slabs = nullptr;          // evaluation form: [score_max_blocks][AGD_EVAL_N]
+  long long row_base = 0;           // evaluation form: global index of the shard's first row ...
+  const RowFilter *filt = nullptr;  // ... and the view whose rows are summed (rows outside it are not even read)
   cudaStream_t stream = nullptr;
 };
 int score_max_blocks(int sm_count);
 cudaError_t score_margins_launch(const ScoreArgs &a, int elem_bytes, int sm_count);
 // *blocks_out = slabs written (0 for an empty range)
 cudaError_t score_eval_launch(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out);
+// out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
+cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);
+// the same predicate as a bitmap: bit i % 32 of bits[i / 32] for rows [0, rows) (ceil(rows / 32) words)
+cudaError_t row_filter_bits_launch(const RowFilter *f, long long row_base, int64_t rows, uint32_t *bits, cudaStream_t st);
 
 
 // ---------------------------------------------------------------- K3: fused O(d) driver-side vector work

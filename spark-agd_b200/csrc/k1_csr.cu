@@ -24,7 +24,7 @@ __device__ __forceinline__ bool csr_row_folds(int kind, bool sel, double mult) {
   return sel && (mult != 0.0 || kind != AGD_GRAD_HINGE);
 }
 
-template <typename T, bool DUAL>
+template <typename T, bool DUAL, bool VIEW>
 __global__ void __launch_bounds__(256) k1_csr_kernel(const K1CsrArgs a) {
   __shared__ double red[32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(256) k1_csr_kernel(const K1CsrArgs a) {
     double mult, loss;
     const double ylab = a.labels[r];
     loss_eval(a.kind, m, ylab, mult, loss);
-    const bool sel = row_selected(a.sample_seed, a.sample_thresh, a.row_base + r);
+    const bool sel = row_kept(a.sample_seed, a.sample_thresh, VIEW ? a.filt : nullptr, a.row_base + r);
     if (!sel) { mult = 0.0; loss = 0.0; }
     else if (lane == 0) cntacc += 1.0;
     if (lane == 0) lossacc += loss;
@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(256) k1_csr_kernel(const K1CsrArgs a) {
 
 // The same fold with more loads in flight (selected by default; option ring_rows=1 keeps the simple loop above): the kernel is
 // bound by the latency of dependent loads, rowptr -> idx/val -> w gather (ncu: 74 % long-scoreboard stalls, L2 at 65 % of peak).
-template <typename T, bool DUAL>
+template <typename T, bool DUAL, bool VIEW>
 __global__ void __launch_bounds__(256) k1_csr_pipelined_kernel(const K1CsrArgs a) {
   __shared__ double red[32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -131,7 +131,7 @@ __global__ void __launch_bounds__(256) k1_csr_pipelined_kernel(const K1CsrArgs a
     }
     double mult, loss;
     loss_eval(a.kind, m, ylab, mult, loss);
-    const bool sel = row_selected(a.sample_seed, a.sample_thresh, a.row_base + r);
+    const bool sel = row_kept(a.sample_seed, a.sample_thresh, VIEW ? a.filt : nullptr, a.row_base + r);
     if (!sel) { mult = 0.0; loss = 0.0; }
     else if (lane == 0) cntacc += 1.0;
     if (lane == 0) lossacc += loss;
@@ -168,30 +168,38 @@ __global__ void __launch_bounds__(256) k1_csr_pipelined_kernel(const K1CsrArgs a
 
 }  // namespace
 
+// VIEW: a launch on a view (a.filt != nullptr).  A launch without one takes the instantiation that has no view code, whose
+// registers and instructions are those of a plain sweep.
+template <bool VIEW>
+static void k1_csr_launch_t(const K1CsrArgs &a, int elem_bytes, unsigned grid, cudaStream_t st) {
+  const bool simple = a.tune == 1;
+  if (elem_bytes == 4) {
+    if (simple) {
+      if (a.w2) k1_csr_kernel<float, true, VIEW><<<grid, 256, 0, st>>>(a);
+      else k1_csr_kernel<float, false, VIEW><<<grid, 256, 0, st>>>(a);
+    } else {
+      if (a.w2) k1_csr_pipelined_kernel<float, true, VIEW><<<grid, 256, 0, st>>>(a);
+      else k1_csr_pipelined_kernel<float, false, VIEW><<<grid, 256, 0, st>>>(a);
+    }
+  } else {
+    if (simple) {
+      if (a.w2) k1_csr_kernel<double, true, VIEW><<<grid, 256, 0, st>>>(a);
+      else k1_csr_kernel<double, false, VIEW><<<grid, 256, 0, st>>>(a);
+    } else {
+      if (a.w2) k1_csr_pipelined_kernel<double, true, VIEW><<<grid, 256, 0, st>>>(a);
+      else k1_csr_pipelined_kernel<double, false, VIEW><<<grid, 256, 0, st>>>(a);
+    }
+  }
+}
+
 cudaError_t k1_csr_launch(const K1CsrArgs &a, int elem_bytes, int sm_count, cudaStream_t st) {
   cudaError_t e = cudaMemsetAsync(a.gacc, 0, ((size_t)a.d + 4) * sizeof(double), st);
   if (e != cudaSuccess) return e;
   long long grid = (a.rows + 7) / 8;
   if (grid > 8LL * sm_count) grid = 8LL * sm_count;
   if (grid < 1) grid = 1;
-  const bool simple = a.tune == 1;
-  if (elem_bytes == 4) {
-    if (simple) {
-      if (a.w2) k1_csr_kernel<float, true><<<(unsigned)grid, 256, 0, st>>>(a);
-      else k1_csr_kernel<float, false><<<(unsigned)grid, 256, 0, st>>>(a);
-    } else {
-      if (a.w2) k1_csr_pipelined_kernel<float, true><<<(unsigned)grid, 256, 0, st>>>(a);
-      else k1_csr_pipelined_kernel<float, false><<<(unsigned)grid, 256, 0, st>>>(a);
-    }
-  } else {
-    if (simple) {
-      if (a.w2) k1_csr_kernel<double, true><<<(unsigned)grid, 256, 0, st>>>(a);
-      else k1_csr_kernel<double, false><<<(unsigned)grid, 256, 0, st>>>(a);
-    } else {
-      if (a.w2) k1_csr_pipelined_kernel<double, true><<<(unsigned)grid, 256, 0, st>>>(a);
-      else k1_csr_pipelined_kernel<double, false><<<(unsigned)grid, 256, 0, st>>>(a);
-    }
-  }
+  if (a.filt) k1_csr_launch_t<true>(a, elem_bytes, (unsigned)grid, st);
+  else k1_csr_launch_t<false>(a, elem_bytes, (unsigned)grid, st);
   return cudaGetLastError();
 }
 

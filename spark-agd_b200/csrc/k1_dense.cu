@@ -148,7 +148,9 @@ __device__ __forceinline__ double warp_rows_reduce_perm(double (&p)[R]) {
 }
 
 // ---------------------------------------------------------------- the hot kernel
-template <typename T, int NT, int TPR, int V, int R, int MINB, int MODE>
+// VIEW: the launch runs on a view (a.filt != nullptr).  Launches without one take the instantiation that has no view code at
+// all, so their registers and instructions are those of a kernel that never heard of views.
+template <typename T, int NT, int TPR, int V, int R, int MINB, int MODE, bool VIEW>
 __global__ void __launch_bounds__(NT, MINB)
 k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uint32_t aux_bytes) {
   constexpr int EPV = Elem<T>::EPV;
@@ -409,7 +411,10 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
 #pragma unroll
       for (int wi = 0; wi < 8; ++wi) pw[wi] = (wi < WPG) ? pp[srow * 8 + wi] : 0.0;
       const double m = ((pw[0] + pw[1]) + (pw[2] + pw[3])) + ((pw[4] + pw[5]) + (pw[6] + pw[7]));
-      row_ok = srow < rv && row_selected(a.sample_seed, a.sample_thresh, a.row_base + row0 + srow);
+      // VIEW: the row's bit of the view bitmap (row_in_view() of every row, drawn once when the filter was set) -- one load,
+      // where the Philox rounds of row_in_view() would need registers this section does not have
+      row_ok = srow < rv && (!VIEW || ((a.view_bits[(row0 + srow) >> 5] >> ((row0 + srow) & 31)) & 1u) != 0u) &&
+               row_selected(a.sample_seed, a.sample_thresh, a.row_base + row0 + srow);
       double mult, loss = 0.0;
       if (a.kind == AGD_GRAD_LOGISTIC) mult = logistic_head(m, ylab, mid);
       else loss_eval(a.kind, m, ylab, mult, loss);
@@ -551,7 +556,7 @@ template <> __device__ __forceinline__ double load_elem<__nv_bfloat16>(const __n
 // ---------------------------------------------------------------- generic shapes
 // a.w2 != nullptr: the loss (not the gradient) is also evaluated at w2 in the same sweep -- threads 32..32+R-1 play the
 // part of threads 0..R-1 for it, so its sum is formed exactly as a launch of its own would form it.
-template <typename T>
+template <typename T, bool VIEW>
 __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const long long ntiles) {
   constexpr int R = 8;
   __shared__ double part[2][R][8];
@@ -602,7 +607,7 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
 #pragma unroll
       for (int wi = 0; wi < 8; ++wi) m += part[which][srow][wi];
       double mult = 0.0, loss = 0.0;
-      if (srow < rv && row_selected(a.sample_seed, a.sample_thresh, a.row_base + row0 + srow)) {
+      if (srow < rv && row_kept(a.sample_seed, a.sample_thresh, VIEW ? a.filt : nullptr, a.row_base + row0 + srow)) {
         loss_eval(a.kind, m, a.labels[row0 + srow], mult, loss);
         cntacc += 1.0;
       }
@@ -748,16 +753,17 @@ cudaError_t launch_ring_inst(const K1Args &a_in, int nvec, int sm_count, int *bl
   a.stages = stages;
   a.slab_stride = (MODE == 2 ? 2 : 1) * (a.d + 4);
   const RingLayout L = ring_layout(tile_bytes, aux_bytes, stages, MODE);
-  auto kern = k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE>;
+  const int view = a.filt ? 1 : 0;
+  auto kern = view ? k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, true> : k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, false>;
   // the opt-in shared-memory size is a per-device property of the function: set it when it changes, not on every launch
-  static int smem_set[64] = {0};
+  static int smem_set[2][64] = {};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64 || smem_set[dev] != (int)L.total) {
+  if (dev < 0 || dev >= 64 || smem_set[view][dev] != (int)L.total) {
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) smem_set[dev] = (int)L.total;
+    if (dev >= 0 && dev < 64) smem_set[view][dev] = (int)L.total;
   }
   const long long ntiles = (a.rows + TR - 1) / TR;
   long long grid = (long long)MINB * sm_count;
@@ -878,9 +884,15 @@ cudaError_t k1_generic_launch(const K1Args &a, int elem_bytes, int sm_count, int
   if (grid > ntiles) grid = ntiles;
   if (grid < 1) grid = 1;
   *blocks_out = (int)grid;
-  if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-  else if (elem_bytes == 4) k1_generic_kernel<float><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-  else k1_generic_kernel<double><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+  if (a.filt) {
+    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+    else if (elem_bytes == 4) k1_generic_kernel<float, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+    else k1_generic_kernel<double, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+  } else {
+    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+    else if (elem_bytes == 4) k1_generic_kernel<float, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+    else k1_generic_kernel<double, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+  }
   return cudaGetLastError();
 }
 

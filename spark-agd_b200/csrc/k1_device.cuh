@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include "../../include/agd_b200.h"
+#include "agd_common.cuh"
 
 namespace agd {
 
@@ -127,13 +128,10 @@ __device__ __forceinline__ void loss_eval(int kind, double m, double y, double &
   }
 }
 
-// Bernoulli row mask of the mini-batch form of runMiniBatchSGD (`data.sample(false, fraction, 42 + i)`):
-// row `grow` (global index) is kept iff the 64-bit Philox4x32-10 draw keyed by `seed`, counter (row, 0, 6) is
-// below `thresh` (= fraction * 2^64; thresh == 0 means "no sampling").  Counter-based, so the mask does not depend
-// on how rows are sharded over GPUs.  (Spark's own sampler is seeded per partition and is not reproducible either.)
-__device__ __forceinline__ bool row_selected(unsigned long long seed, unsigned long long thresh, long long grow) {
-  if (thresh == 0ull) return true;
-  uint32_t c0 = (uint32_t)grow, c1 = (uint32_t)((unsigned long long)grow >> 32), c2 = 0u, c3 = 6u;
+// The 64-bit per-row draw: Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, stream), output words 0 and 1.
+// Streams 1-5 belong to the synthetic generator (synth.cu), 6 to the mini-batch mask, 7 to views.
+__device__ __forceinline__ unsigned long long row_draw(unsigned long long seed, long long grow, uint32_t stream) {
+  uint32_t c0 = (uint32_t)grow, c1 = (uint32_t)((unsigned long long)grow >> 32), c2 = 0u, c3 = stream;
   uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -143,7 +141,41 @@ __device__ __forceinline__ bool row_selected(unsigned long long seed, unsigned l
     c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
-  return (((unsigned long long)c0 << 32) | c1) < thresh;
+  return ((unsigned long long)c0 << 32) | c1;
+}
+
+// Bernoulli row mask of the mini-batch form of runMiniBatchSGD (`data.sample(false, fraction, 42 + i)`):
+// row `grow` (global index) is kept iff its stream-6 draw is below `thresh` (= fraction * 2^64; thresh == 0 means
+// "no sampling").  Counter-based, so the mask does not depend on how rows are sharded over GPUs.  (Spark's own
+// sampler is seeded per partition and is not reproducible either.)
+__device__ __forceinline__ bool row_selected(unsigned long long seed, unsigned long long thresh, long long grow) {
+  if (thresh == 0ull) return true;
+  return row_draw(seed, grow, 6u) < thresh;
+}
+
+// Whether row `grow` belongs to the view `f` (agd_set_row_filter): every predicate i must hold on the row's stream-7
+// draw u = row_draw(seed_i, grow, 7), i.e. lo_i <= u < hi_i, negated when complemented.  f == nullptr returns before any
+// arithmetic, so a call without a view runs the instructions it ran before views existed.  The predicates are read from
+// device memory inside the row loop (one rolled loop, L1 hits) rather than held in registers: the callers' register
+// budgets stay what they were.
+__device__ __forceinline__ bool row_in_view(const RowFilter *f, long long grow) {
+  if (f == nullptr) return true;
+  const int n = f->n;
+  bool keep = true;
+#pragma unroll 1
+  for (int i = 0; i < n; ++i) {
+    const unsigned long long u = row_draw(f->seed[i], grow, 7u);
+    const uint32_t fl = f->flags[i];
+    const bool in = ((fl & kRowPredLoEnd) == 0u && u >= f->lo[i]) && ((fl & kRowPredHiEnd) != 0u || u < f->hi[i]);
+    keep = keep && (in != ((fl & kRowPredComplement) != 0u));
+  }
+  return keep;
+}
+
+// The row rule of every gradient sweep: inside the view, and kept by the mini-batch mask
+__device__ __forceinline__ bool row_kept(unsigned long long seed, unsigned long long thresh, const RowFilter *f,
+                                         long long grow) {
+  return row_selected(seed, thresh, grow) && row_in_view(f, grow);
 }
 
 // Transpose-reduce R per-lane partials across a warp: afterwards every lane holds the warp total of

@@ -163,7 +163,9 @@ struct TcArgs {
   int d, kind, slab_stride;
   unsigned long long sample_seed, sample_thresh;
   long long row_base;
-  int gb;           // 64-feature blocks per ring group: the largest even divisor of d / 64 that is <= 8
+  const RowFilter *filt;   // the view (nullptr: every row) ...
+  const uint32_t *view_bits;  // ... as a bitmap of the shard's rows (K1Args::view_bits)
+  int gb;                  // 64-feature blocks per ring group: the largest even divisor of d / 64 that is <= 8
   int ngt;          // groups per tile = d / (64 * gb)
   int ring_groups;  // ring capacity in groups
   int one_copy;     // 1: a ring group arrives as ONE 3-D TMA copy [gb blocks][16 rows][64 features] instead of gb 2-D copies
@@ -195,7 +197,8 @@ __device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
 // DUAL == 2: the GRADIENT at w2 as well (two-gradient sweep): r at w2 takes columns 2j+9, 16+2j and 17+2j of a 24-column B
 // operand (hi2, mid2, lo2 for lane j of a quad), so the second X^T r costs no extra MMA instruction; its fp64 gradient
 // lives in shared memory (g2), each entry owned by the one MMA thread that updates it.
-template <int RPT, bool F32, int DUAL = 0>
+// VIEW: the launch runs on a view (a.filt != nullptr); launches without one take the instantiation without view code.
+template <int RPT, bool F32, int DUAL, bool VIEW>
 __global__ void __launch_bounds__(tc_consumers(RPT) + 256, 1)
 k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap3, const TcArgs a,
              const long long ntiles) {
@@ -298,7 +301,10 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
         nonfinite = (lane < kKR || DUAL == 2) && srow < rv && !isfinite(m);
         double mu, loss;
         loss_eval(a.kind, m, ylab, mu, loss);
-        if (srow < rv && row_selected(a.sample_seed, a.sample_thresh, a.row_base + tile * kKR + srow)) {
+        // VIEW: the row's bit of the view bitmap (drawn by row_in_view() when the filter was set): one load, where the Philox
+        // rounds would need registers the two-gradient form does not have
+        if (srow < rv && (!VIEW || ((a.view_bits[(tile * kKR + srow) >> 5] >> ((tile * kKR + srow) & 31)) & 1u) != 0u) &&
+            row_selected(a.sample_seed, a.sample_thresh, a.row_base + tile * kKR + srow)) {
           mult = mu; lossacc += loss; cntacc += 1.0;
         }
       }
@@ -683,6 +689,39 @@ cudaError_t set_smem_once(K kern, int bytes) {
   return e;
 }
 
+// the kernel form of a launch (options, second point), with or without view code
+template <bool VIEW>
+cudaError_t tc_launch_forms(const K1Args &a, const CUtensorMap &tmap, const CUtensorMap &tmap3, const TcArgs &t, long long grid,
+                            int smem_bytes, long long ntiles, cudaStream_t st) {
+  cudaError_t e;
+  if (a.tune_rows == 1) {  // option ring_rows=1: row-per-lane consumers (broadcast w reads; measured slower)
+    e = set_smem_once<1 + 8 * VIEW>(k1_tc_kernel<0, false, 0, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<0, false, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  } else if (a.tune_rows == 4) {  // option ring_rows=4: 256 consumers with four rows each (measured slower)
+    e = set_smem_once<2 + 8 * VIEW>(k1_tc_kernel<4, false, 0, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<4, false, 0, VIEW><<<(unsigned)grid, 512, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  } else if (a.tc_margins_f64) {  // option tc_margins=f64: 512 consumers, two rows per thread, fp64-exact margins
+    e = set_smem_once<3 + 8 * VIEW>(k1_tc_kernel<2, false, 0, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<2, false, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  } else if (a.w2 && a.dual_full) {  // the default mapping + loss AND gradient at a second point (speculative sweep)
+    e = set_smem_once<6 + 8 * VIEW>(k1_tc_kernel<2, true, 2, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<2, true, 2, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  } else if (a.w2) {  // the default mapping + the loss at a second point (pass fusion)
+    e = set_smem_once<4 + 8 * VIEW>(k1_tc_kernel<2, true, 1, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<2, true, 1, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  } else {  // default: the same mapping with fp32 phase-1 arithmetic (fp32 FMAs on packed pairs, no fp64 conversion per element)
+    e = set_smem_once<5 + 8 * VIEW>(k1_tc_kernel<2, true, 0, VIEW>, smem_bytes);
+    if (e != cudaSuccess) return e;
+    k1_tc_kernel<2, true, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+  }
+  return cudaGetLastError();
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -733,7 +772,7 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
   if (a.w2 && (a.tune_rows != 0 || a.tc_margins_f64)) return cudaErrorInvalidValue;   // two-point form: default mapping only
   t.labels = a.labels; t.w = a.w; t.w2 = a.w2; t.slabs = a.slabs; t.rows = a.rows; t.d = a.d; t.kind = a.kind;
   t.slab_stride = a.slab_stride;
-  t.sample_seed = a.sample_seed; t.sample_thresh = a.sample_thresh; t.row_base = a.row_base;
+  t.sample_seed = a.sample_seed; t.sample_thresh = a.sample_thresh; t.row_base = a.row_base; t.filt = a.filt; t.view_bits = a.view_bits;
   t.gb = gb;
   t.ngt = nblk / gb;
   const int group_bytes = t.gb * kBlockBytes;
@@ -750,33 +789,8 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
   if (grid > ntiles) grid = ntiles;
   *blocks_out = (int)grid;
   const int smem_bytes = (int)L.total + 1024;
-  cudaError_t e;
-  if (a.tune_rows == 1) {  // option ring_rows=1: row-per-lane consumers (broadcast w reads; measured slower)
-    e = set_smem_once<1>(k1_tc_kernel<0, false, 0>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<0, false, 0><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else if (a.tune_rows == 4) {  // option ring_rows=4: 256 consumers with four rows each (measured slower)
-    e = set_smem_once<2>(k1_tc_kernel<4, false, 0>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<4, false, 0><<<(unsigned)grid, 512, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else if (a.tc_margins_f64) {  // option tc_margins=f64: 512 consumers, two rows per thread, fp64-exact margins
-    e = set_smem_once<3>(k1_tc_kernel<2, false, 0>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, false, 0><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else if (a.w2 && a.dual_full) {  // the default mapping + loss AND gradient at a second point (speculative sweep)
-    e = set_smem_once<6>(k1_tc_kernel<2, true, 2>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 2><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else if (a.w2) {  // the default mapping + the loss at a second point (pass fusion)
-    e = set_smem_once<4>(k1_tc_kernel<2, true, 1>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 1><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  } else {  // default: the same mapping with fp32 phase-1 arithmetic (fp32 FMAs on packed pairs, no fp64 conversion per element)
-    e = set_smem_once<5>(k1_tc_kernel<2, true, 0>, smem_bytes);
-    if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 0><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
-  }
-  return cudaGetLastError();
+  return a.filt ? tc_launch_forms<true>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st)
+                : tc_launch_forms<false>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st);
 }
 
 }  // namespace agd

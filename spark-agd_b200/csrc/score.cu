@@ -15,6 +15,8 @@
 //     one slab per CTA; k1_reduce_launch then adds the slabs in a fixed order, so repeated calls return identical bits
 //     (also on CSR shards, where K1 scatters with RED.ADD).
 // Non-finite features follow IEEE arithmetic: nothing is skipped (0 * inf = NaN, as ddot gives).
+// On a view (agd_set_row_filter) the evaluation form treats a row outside it as past the end of the shard: its loads are
+// never issued, so it leaves no trace in the sums, and a held-out view reads only its own rows' lines of X.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -154,7 +156,7 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_dense_kernel(const Sco
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       row[r] = base + (long long)r * groups + g;
-      ok[r] = row[r] < a.rows;
+      ok[r] = row[r] < a.rows && (!EVAL || row_in_view(a.filt, a.row_base + a.row0 + row[r]));
       acc[r] = 0.0;
     }
     const T *xr[R];
@@ -231,7 +233,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_csr_kernel(const ScoreArg
   for (int k = 0; k < AGD_EVAL_N; ++k) s[k] = 0.0;
   for (long long base = warp0 * groups; base < a.rows; base += nwarps * groups) {
     const long long row = base + g;
-    const bool ok = row < a.rows;
+    const bool ok = row < a.rows && (!EVAL || row_in_view(a.filt, a.row_base + a.row0 + row));
     double acc = 0.0;
     if (ok) {
       const long long r = a.row0 + row;
@@ -307,7 +309,40 @@ cudaError_t launch_any(const ScoreArgs &a, int elem_bytes, int sm_count, int *bl
   return cudaErrorInvalidValue;
 }
 
+// which rows of a range pass a view: the predicate the K1 and evaluation sweeps apply, one row per thread
+__global__ void __launch_bounds__(kScoreThreads) row_filter_mask_kernel(const RowFilter *f, long long row_base, int64_t rows,
+                                                                       uint8_t *out) {
+  for (long long i = blockIdx.x * (long long)kScoreThreads + threadIdx.x; i < rows; i += (long long)gridDim.x * kScoreThreads)
+    out[i] = row_in_view(f, row_base + i) ? 1 : 0;
+}
+
+// the same predicate packed 32 rows to a word: one row per thread, a warp's ballot is one word
+__global__ void __launch_bounds__(kScoreThreads) row_filter_bits_kernel(const RowFilter *f, long long row_base, int64_t rows,
+                                                                       uint32_t *bits) {
+  const long long stride = (long long)gridDim.x * kScoreThreads;
+  for (long long i = blockIdx.x * (long long)kScoreThreads + threadIdx.x; i - (threadIdx.x & 31) < rows; i += stride) {
+    const uint32_t word = __ballot_sync(0xffffffffu, i < rows && row_in_view(f, row_base + i));
+    if ((threadIdx.x & 31) == 0) bits[i >> 5] = word;
+  }
+}
+
 }  // namespace
+
+cudaError_t row_filter_bits_launch(const RowFilter *f, long long row_base, int64_t rows, uint32_t *bits, cudaStream_t st) {
+  if (rows <= 0) return cudaSuccess;
+  long long grid = (rows + kScoreThreads - 1) / kScoreThreads;
+  if (grid > 4096) grid = 4096;
+  row_filter_bits_kernel<<<(unsigned)grid, kScoreThreads, 0, st>>>(f, row_base, rows, bits);
+  return cudaGetLastError();
+}
+
+cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st) {
+  if (rows <= 0) return cudaSuccess;
+  long long grid = (rows + kScoreThreads - 1) / kScoreThreads;
+  if (grid > 4096) grid = 4096;
+  row_filter_mask_kernel<<<(unsigned)grid, kScoreThreads, 0, st>>>(f, row_base, rows, out);
+  return cudaGetLastError();
+}
 
 int score_max_blocks(int sm_count) { return 8 * sm_count; }
 

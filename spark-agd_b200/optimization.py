@@ -188,18 +188,124 @@ def _synthetic_csr(ctx, total_rows, d, nnz_per_row, gradient, seed=42, store="f3
 Context.synthetic_csr = _synthetic_csr
 
 
+# Views (randomSplit / sample / kFold): a predicate (seed, lo, hi, complement) keeps row r iff lo <= u(seed, r) < hi on the
+# row's own 64-bit Philox draw (include/agd_b200.h, agd_set_row_filter), negated when complemented; a view keeps the rows
+# every one of its predicates keeps.  Every rank of a world must select the same rows, so the default seed is fixed, not
+# random.
+DEFAULT_SPLIT_SEED = 42
+MAX_VIEW_PREDICATES = 4
+
+
+def split_bounds(weights) -> list:
+    """RDD.randomSplit's cell bounds: the weights normalised by their sum and accumulated in fp64
+    (weights.map(_ / sum).scanLeft(0.0)(_ + _)).  The last bound is 1, so rounding in the sum can leave no row out."""
+    w = [float(x) for x in weights]
+    if not w:
+        raise ValueError("randomSplit needs at least one weight")
+    if any(not (x >= 0.0) or x == float("inf") for x in w):
+        raise ValueError(f"weights must be finite and nonnegative, got {weights}")
+    total = sum(w)
+    if not (total > 0.0):
+        raise ValueError(f"sum of weights must be positive, got {weights}")
+    bounds = [0.0]
+    for x in w:
+        bounds.append(bounds[-1] + x / total)
+    bounds = [min(b, 1.0) for b in bounds]
+    bounds[-1] = 1.0
+    return bounds
+
+
 class DeviceDataset:
-    """RDD[(Double, Vector)] stand-in: row shards pinned in HBM for the lifetime of the object."""
+    """RDD[(Double, Vector)] stand-in: row shards pinned in HBM for the lifetime of the object.
+
+    randomSplit / sample / MLUtils.kFold return views: DeviceDatasets that share this one's shards and handle and select
+    rows by a fixed predicate on each row's own random draw, without copying a row.  Every compute call on a view (smooth*,
+    evaluate, margins, training) sets the view's filter on the handle for that call only; close() on a view frees nothing.
+    The accessors that address PHYSICAL rows -- local_rows, get_rows, get_labels, get_csr_rows, margins_rows -- return the
+    parent's rows on a view as well (the view's own rows of them: row_mask; its row count: count())."""
 
     def __init__(self, ctx: Context):
         self.ctx = ctx
         self.h = ctx._new_handle()
         self.total_rows = 0
         self._xchg_d = 0       # dimension the host-shipped exchange (transport="ipc") was set up for
+        self._base = None      # a view: the dataset that owns the shards (kept alive by this reference)
+        self._preds = ()       # a view: its predicates (seed, lo, hi, complement)
+
+    def _view(self, pred) -> "DeviceDataset":
+        preds = self._preds + (pred,)
+        if len(preds) > MAX_VIEW_PREDICATES:
+            raise ValueError(f"a view nests at most {MAX_VIEW_PREDICATES} predicates (randomSplit / sample / kFold levels)")
+        seed, lo, hi, comp = pred
+        if not (0.0 <= lo <= hi <= 1.0):
+            raise ValueError(f"bounds must satisfy 0 <= lo <= hi <= 1, got [{lo}, {hi})")
+        v = object.__new__(DeviceDataset)
+        v.ctx = self.ctx
+        v._base = self._base if self._base is not None else self
+        v.h = v._base.h
+        v.total_rows = v._base.total_rows
+        v._xchg_d = 0
+        v._preds = preds
+        return v
+
+    @property
+    def is_view(self) -> bool:
+        return self._base is not None
+
+    def _filtered(self):
+        """Context manager: the view's filter is on the handle for the duration of one call, and cleared afterwards, also on
+        error (the parent and sibling views never see it).  A dataset that is not a view leaves the handle alone."""
+        ds = self
+
+        class _F:
+            def __enter__(self_):
+                if ds._preds:
+                    n = len(ds._preds)
+                    seeds = np.array([p[0] for p in ds._preds], dtype=np.uint64)
+                    lo = np.array([p[1] for p in ds._preds], dtype=np.float64)
+                    hi = np.array([p[2] for p in ds._preds], dtype=np.float64)
+                    comp = np.array([1 if p[3] else 0 for p in ds._preds], dtype=np.int32)
+                    N.check(N.lib().agd_set_row_filter(ds.h, n, _ptr(seeds), _ptr(lo), _ptr(hi), _ptr(comp)), ds.h)
+
+            def __exit__(self_, *exc):
+                if ds._preds:
+                    N.check(N.lib().agd_set_row_filter(ds.h, 0, None, None, None, None), ds.h)
+                return False
+
+        return _F()
+
+    # --- views (RDD.randomSplit, RDD.sample, MLUtils.kFold) ---
+    def randomSplit(self, weights, seed: int = DEFAULT_SPLIT_SEED) -> list:
+        """RDD.randomSplit(weights, seed): disjoint views that cover every row; split k keeps the rows whose draw lies in
+        [c_k, c_{k+1}) of the normalised cumulative weights (split_bounds)."""
+        b = split_bounds(weights)
+        return [self._view((int(seed), b[k], b[k + 1], False)) for k in range(len(b) - 1)]
+
+    def sample(self, withReplacement: bool, fraction: float, seed: int = DEFAULT_SPLIT_SEED) -> "DeviceDataset":
+        """RDD.sample(False, fraction, seed): a Bernoulli view keeping the rows whose draw lies in [0, fraction)."""
+        if withReplacement:
+            raise NotImplementedError("sample(withReplacement=True) needs per-row multiplicities; only Bernoulli views exist")
+        fraction = float(fraction)
+        if not (0.0 <= fraction <= 1.0):
+            raise ValueError(f"fraction must be in [0, 1] without replacement, got {fraction}")
+        return self._view((int(seed), 0.0, fraction, False))
+
+    def count(self) -> int:
+        """Rows of this dataset (or view) over every shard of the world (collective: one evaluation sweep)."""
+        return int(self.evaluate(LeastSquaresGradient(), np.zeros(self.d)).count)
+
+    def row_mask(self, dev: int, row0: int, rows: int) -> np.ndarray:
+        """Which physical rows [row0, row0 + rows) of local device `dev`'s shard this view keeps (bool; rank-local)."""
+        out = np.empty(max(int(rows), 0), dtype=np.uint8)
+        with self._filtered():
+            N.check(N.lib().agd_row_filter_mask(self.h, dev, int(row0), int(rows), _ptr(out) if rows > 0 else None), self.h)
+        return out.astype(bool)
 
     def _ensure_exchange(self):
         """transport="ipc": ship the CUDA IPC handles of the exchange buffers once per loaded dimension (collective:
         every process reaches this from the same compute call)."""
+        if self._base is not None:
+            return self._base._ensure_exchange()
         c = self.ctx
         if c.transport != "ipc" or c.world_size <= len(c.devices) or self._xchg_d == self.d:
             return
@@ -217,12 +323,18 @@ class DeviceDataset:
 
     def unpersist(self) -> "DeviceDataset":
         """Drops every shard but keeps the context (devices, communicator) for the next load."""
+        self._no_view("unpersist")
         N.check(N.lib().agd_clear(self.h), self.h)
         self.total_rows = 0
         self._xchg_d = 0
         return self
 
+    def _no_view(self, what: str):
+        if self._base is not None:
+            raise ValueError(f"{what} changes the shards; a view shares its parent's and cannot")
+
     def load_dense(self, labels, X, store: str = "f64"):
+        self._no_view("load_dense")
         labels = np.ascontiguousarray(labels, dtype=np.float64)
         X = np.asarray(X)
         if X.dtype not in _DT:
@@ -242,6 +354,7 @@ class DeviceDataset:
         self.total_rows += n
 
     def load_csr(self, labels, rowptr, idx, val, d: int, store: str = "f64"):
+        self._no_view("load_csr")
         labels = np.ascontiguousarray(labels, dtype=np.float64)
         rowptr = np.ascontiguousarray(rowptr, dtype=np.int64)
         idx = np.ascontiguousarray(idx, dtype=np.int32)
@@ -264,16 +377,19 @@ class DeviceDataset:
         return int(N.lib().agd_dim(self.h))
 
     def local_rows(self, dev: int = 0) -> int:
+        """Physical rows of local device `dev`'s shard (on a view too: the parent's)."""
         return int(N.lib().agd_rows(self.h, dev))
 
     def get_rows(self, dev: int, row0: int, rows: int, dtype=np.float32):
-        """Rows as stored (dtype must match the storage: float32, float64, or uint16 for raw bf16)."""
+        """Physical rows as stored (dtype must match the storage: float32, float64, or uint16 for raw bf16); on a view, the
+        parent's rows [row0, row0 + rows) -- select the view's with row_mask(dev, row0, rows)."""
         X = np.empty((rows, self.d), dtype=dtype)
         y = np.empty(rows, dtype=np.float64)
         N.check(N.lib().agd_get_rows(self.h, dev, row0, rows, _ptr(X), _ptr(y)), self.h)
         return X, y
 
     def get_labels(self, dev: int, row0: int, rows: int) -> np.ndarray:
+        """Labels of physical rows [row0, row0 + rows) (on a view too, as get_rows)."""
         y = np.empty(rows, dtype=np.float64)
         N.check(N.lib().agd_get_rows(self.h, dev, row0, rows, None, _ptr(y)), self.h)
         return y
@@ -283,6 +399,7 @@ class DeviceDataset:
         return (N.lib().agd_kernel_name(self.h, dev) or b"").decode()
 
     def get_csr_rows(self, dev: int, row0: int, rows: int, nnz_capacity: int, dtype=np.float32):
+        """Physical CSR rows [row0, row0 + rows) (on a view too, as get_rows)."""
         rowptr = np.empty(rows + 1, dtype=np.int64)
         idx = np.empty(nnz_capacity, dtype=np.int32)
         val = np.empty(nnz_capacity, dtype=dtype)
@@ -304,7 +421,8 @@ class DeviceDataset:
         g = np.empty(self.d, dtype=np.float64)
         loss, cnt = C.c_double(), C.c_int64()
         self._ensure_exchange()
-        N.check(N.lib().agd_smooth(self.h, _grad_kind(gradient), _ptr(w), C.byref(loss), _ptr(g), C.byref(cnt)), self.h)
+        with self._filtered():
+            N.check(N.lib().agd_smooth(self.h, _grad_kind(gradient), _ptr(w), C.byref(loss), _ptr(g), C.byref(cnt)), self.h)
         return loss.value, g, cnt.value
 
     def smooth_pair(self, gradient: Gradient, w, w2):
@@ -317,8 +435,9 @@ class DeviceDataset:
         g = np.empty(self.d, dtype=np.float64)
         loss, loss2, cnt = C.c_double(), C.c_double(), C.c_int64()
         self._ensure_exchange()
-        N.check(N.lib().agd_smooth_pair(self.h, _grad_kind(gradient), _ptr(w), _ptr(w2), C.byref(loss), _ptr(g),
-                                        C.byref(cnt), C.byref(loss2)), self.h)
+        with self._filtered():
+            N.check(N.lib().agd_smooth_pair(self.h, _grad_kind(gradient), _ptr(w), _ptr(w2), C.byref(loss), _ptr(g),
+                                            C.byref(cnt), C.byref(loss2)), self.h)
         return loss.value, g, cnt.value, loss2.value
 
     def smooth_two(self, gradient: Gradient, w, w2):
@@ -330,8 +449,9 @@ class DeviceDataset:
         g, g2 = np.empty(self.d, dtype=np.float64), np.empty(self.d, dtype=np.float64)
         loss, loss2, cnt = C.c_double(), C.c_double(), C.c_int64()
         self._ensure_exchange()
-        N.check(N.lib().agd_smooth_two(self.h, _grad_kind(gradient), _ptr(w), _ptr(w2), C.byref(loss), _ptr(g),
-                                       C.byref(cnt), C.byref(loss2), _ptr(g2)), self.h)
+        with self._filtered():
+            N.check(N.lib().agd_smooth_two(self.h, _grad_kind(gradient), _ptr(w), _ptr(w2), C.byref(loss), _ptr(g),
+                                           C.byref(cnt), C.byref(loss2), _ptr(g2)), self.h)
         return loss.value, g, cnt.value, loss2.value, g2
 
     # scoring the resident shards (no host copy of X)
@@ -342,16 +462,21 @@ class DeviceDataset:
         return w
 
     def margins_rows(self, dev: int, row0: int, rows: int, w, intercept: float = 0.0) -> np.ndarray:
-        """x_i . w + intercept (fp64) of rows [row0, row0 + rows) of local device `dev`'s shard (not collective)."""
+        """x_i . w + intercept (fp64) of physical rows [row0, row0 + rows) of local device `dev`'s shard (not collective; on a
+        view too, see margins for the view's rows)."""
         w = self._weights(w)
         out = np.empty(max(int(rows), 0), dtype=np.float64)
         N.check(N.lib().agd_margins(self.h, dev, _ptr(w), float(intercept), int(row0), int(rows), _ptr(out)), self.h)
         return out
 
     def margins(self, w, intercept: float = 0.0) -> np.ndarray:
-        """x_i . w + intercept (fp64) of this process's rows, across its local devices in load order (not collective)."""
-        return np.concatenate([self.margins_rows(i, 0, self.local_rows(i), w, intercept)
-                               for i in range(len(self.ctx.devices))])
+        """x_i . w + intercept (fp64) of this process's rows, across its local devices in load order (not collective); on a
+        view, of the view's rows only, in the same order."""
+        parts = []
+        for i in range(len(self.ctx.devices)):
+            m = self.margins_rows(i, 0, self.local_rows(i), w, intercept)
+            parts.append(m[self.row_mask(i, 0, m.shape[0])] if self._preds else m)
+        return np.concatenate(parts)
 
     def evaluate(self, gradient: Gradient, w, intercept: float = 0.0, threshold: float = 0.5) -> "Evaluation":
         """Loss, confusion counts and error moments of the model (w, intercept) over every shard of the world, from one
@@ -359,8 +484,9 @@ class DeviceDataset:
         w = self._weights(w)
         sums = np.empty(N.EVAL_N, dtype=np.float64)
         self._ensure_exchange()
-        N.check(N.lib().agd_evaluate(self.h, _grad_kind(gradient), _ptr(w), float(intercept), float(threshold), _ptr(sums)),
-                self.h)
+        with self._filtered():
+            N.check(N.lib().agd_evaluate(self.h, _grad_kind(gradient), _ptr(w), float(intercept), float(threshold),
+                                         _ptr(sums)), self.h)
         return Evaluation.from_sums(sums)
 
     def prox(self, updater: Updater, w, g, step: float, reg: float):
@@ -374,6 +500,8 @@ class DeviceDataset:
         return rv.value, out
 
     def close(self):
+        if self._base is not None:   # a view owns nothing; dropping it leaves the parent's shards alone
+            return
         if self.h is not None:
             N.lib().agd_destroy(self.h)
             self.h = None
@@ -418,6 +546,19 @@ class MLUtils:
         N.check(N.lib().agd_load_libsvm(ds.h, path.encode(), numFeatures, _STORE[store]), ds.h)
         ds.total_rows = sum(ds.local_rows(i) for i in range(len(sc.devices)))
         return ds
+
+    @staticmethod
+    def kFold(data: "DeviceDataset", numFolds: int, seed: int = DEFAULT_SPLIT_SEED) -> list:
+        """MLUtils.kFold(rdd, numFolds, seed): numFolds (training, validation) pairs of views; validation i keeps the rows
+        whose draw lies in [i / k, (i + 1) / k), training i is its complement."""
+        k = int(numFolds)
+        if k < 2:
+            raise ValueError(f"kFold needs numFolds >= 2, got {numFolds}")
+        out = []
+        for i in range(k):
+            lo, hi = i / k, (i + 1) / k
+            out.append((data._view((int(seed), lo, hi, True)), data._view((int(seed), lo, hi, False))))
+        return out
 
 
 def _ratio(a: float, b: float) -> float:
@@ -571,7 +712,8 @@ def run_with_stats(data: DeviceDataset, gradient, updater, convergenceTol, numIt
     hist = np.empty(max(int(numIterations), 1), dtype=np.float64)
     nh, st = C.c_int32(), N.Stats()
     data._ensure_exchange()
-    N.check(N.lib().agd_run(data.h, C.byref(p), _ptr(w0), _ptr(w), _ptr(hist), C.byref(nh), C.byref(st)), data.h)
+    with data._filtered():
+        N.check(N.lib().agd_run(data.h, C.byref(p), _ptr(w0), _ptr(w), _ptr(hist), C.byref(nh), C.byref(st)), data.h)
     return w, hist[:nh.value].copy(), _stats(st)
 
 
@@ -591,7 +733,8 @@ class GradientDescent:
         hist = np.empty(max(int(numIterations), 1), dtype=np.float64)
         nh, st = C.c_int32(), N.Stats()
         data._ensure_exchange()
-        N.check(N.lib().agd_gd_run_minibatch(data.h, _grad_kind(gradient), _upd_kind(updater), stepSize,
-                                             int(numIterations), regParam, float(miniBatchFraction), _ptr(w0), _ptr(w),
-                                             _ptr(hist), C.byref(nh), C.byref(st)), data.h)
+        with data._filtered():
+            N.check(N.lib().agd_gd_run_minibatch(data.h, _grad_kind(gradient), _upd_kind(updater), stepSize,
+                                                 int(numIterations), regParam, float(miniBatchFraction), _ptr(w0), _ptr(w),
+                                                 _ptr(hist), C.byref(nh), C.byref(st)), data.h)
         return w, hist[:nh.value].copy()
