@@ -205,6 +205,16 @@ int agd_margins(agd_handle *h, int32_t dev, const double *w, double intercept, i
 enum { AGD_EVAL_COUNT = 0, AGD_EVAL_LOSS, AGD_EVAL_TP, AGD_EVAL_FP, AGD_EVAL_TN, AGD_EVAL_FN,
        AGD_EVAL_SUM_ERR, AGD_EVAL_SUM_ERR2, AGD_EVAL_SUM_ABS_ERR, AGD_EVAL_SUM_Y, AGD_EVAL_SUM_Y2, AGD_EVAL_N };
 int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double intercept, double threshold, double *out);
+/* Column statistics over ALL shards of the world (Statistics.colStats; collective, like agd_evaluate): *count = rows in the
+ * view, out = AGD_COLSTAT_N x agd_dim(h) doubles, statistic-major (out[k * agd_dim(h) + j]).  Zeros count as values
+ * (explicit zeros, a CSR row's implicit zeros, zeros of dense rows); padded columns are not reported.  SUM = sum x,
+ * SUM_SQ = sum x^2, SUM_ABS = sum |x|, NNZ = entries with x != 0 (a NaN is nonzero), DEV / DEV2 = sum (x - mu) and
+ * sum (x - mu)^2 with mu = fl(SUM / count) (the unbiased variance is (DEV2 - DEV^2 / count) / (count - 1)), MAX / MIN over
+ * every value, NaN ignored (NaN when every value is NaN).  Two reads of X; sums follow IEEE arithmetic.  Identical bits on
+ * every rank; dense shards also on every repeated call (CSR sums are scattered: equal to rounding). */
+enum { AGD_COLSTAT_SUM = 0, AGD_COLSTAT_SUM_SQ, AGD_COLSTAT_SUM_ABS, AGD_COLSTAT_NNZ,
+       AGD_COLSTAT_DEV, AGD_COLSTAT_DEV2, AGD_COLSTAT_MAX, AGD_COLSTAT_MIN, AGD_COLSTAT_N };
+int agd_col_stats(agd_handle *h, double *count, double *out);
 
 /* ---- views of the resident shards (RDD.randomSplit / sample / MLUtils.kFold without copying a row) ----
  * Every row has a 64-bit draw u = Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, 7), words 0 and 1, where grow
@@ -213,7 +223,7 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask) and agd_evaluate, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate and agd_col_stats, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */

@@ -12,6 +12,7 @@ from .glm import (GeneralizedLinearAlgorithm, GeneralizedLinearModel, LinearRegr
 from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
                            HingeGradient, L1Updater, LeastSquaresGradient, LogisticGradient, MLUtils, RunStats,
                            SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, run_with_stats, split_bounds)
+from .stat import MultivariateStatisticalSummary, Statistics
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -19,4 +20,4 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "GradientDescent",
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
-           "DEFAULT_SPLIT_SEED", "split_bounds"]
+           "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics"]

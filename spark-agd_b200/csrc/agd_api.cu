@@ -89,6 +89,8 @@ struct Dev {
   double *slabs = nullptr;
   size_t slabs_doubles = 0;
   double *eval = nullptr;          // AGD_EVAL_N sums of agd_evaluate (this shard's, then the world's)
+  double *cs = nullptr;            // agd_col_stats: pass-1 sums, maxima, pass-2 sums, CSR max keys (see colstats_layout)
+  size_t cs_doubles = 0;
   double *partials = nullptr;
   unsigned int *ticket = nullptr;
   double *scalars_dev = nullptr;   // device alias of scalars_host: K3 writes its scalars straight to the host
@@ -901,7 +903,7 @@ int agd_destroy(agd_handle *h) {
     if (D.comm && nccl_api().ok) nccl_api().CommDestroy(D.comm);
     D.comm = nullptr;
     free_shard(h, D);
-    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval};
+    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval, D.cs};
     for (double *p : v)
       if (p) cudaFree(p);
     if (D.ticket) cudaFree(D.ticket);
@@ -1488,6 +1490,149 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
   CK(cudaSetDevice(D0.ordinal));
   CK(cudaMemcpyAsync(out, D0.eval, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
   for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  return 0;
+}
+
+// ---------------------------------------------------------------- column statistics (colstats.cu)
+// D.cs, in doubles: [pass-1 sums col_sum_n(d) | maxima 2 d | pass-2 sums 2 d | CSR max keys 2 d]
+struct ColStatsLayout {
+  size_t sums, max, dev, keys, total;
+};
+static ColStatsLayout colstats_layout(int32_t d) {
+  ColStatsLayout L;
+  L.sums = 0;
+  L.max = col_sum_n(d);
+  L.dev = L.max + 2 * (size_t)d;
+  L.keys = L.dev + 2 * (size_t)d;
+  L.total = L.keys + 2 * (size_t)d;
+  return L;
+}
+
+// The all-reduce of n doubles at D.cs + off on every local device (sum, or NaN-ignoring max): epochs of the peer-memory
+// exchange of at most one slot stride each (one-shot or reduce-scatter form by the epoch's size), or one NCCL all-reduce.
+static int colstats_allreduce(agd_handle *h, size_t off, size_t n, int op) {
+  if (h->world <= 1 || n == 0) return 0;
+  const int32_t d = h->d;
+  if (h->x_p2p) {
+    const size_t S = (size_t)xchg_slot_stride(d);
+    for (size_t c0 = 0; c0 < n; c0 += S) {
+      const int m = (int)(n - c0 < S ? n - c0 : S);
+      const bool rs = m >= kXchgRsMin;
+      const unsigned long long epoch = ++h->x_epoch;
+      for (size_t i = 0; i < h->devs.size(); ++i) {
+        Dev &D = h->devs[i];
+        CK(cudaSetDevice(D.ordinal));
+        if (rs) {
+          XchgRs x;
+          x.peers = D.xpeers; x.world = h->world; x.my_rank = h->first_rank + (int)i; x.buf = (int)(epoch & 1ull);
+          x.n = m; x.slot_stride = (int)S; x.epoch = epoch; x.ticket = D.xticket;
+          CK(xchg_rs_publish_launch(D.cs + off + c0, x, D.st));
+          CK(xchg_rs_reduce_bcast_launch(D.xbuf, D.xflags, x, D.st, op));
+        } else {
+          XchgPub pub;
+          pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
+          pub.n = m; pub.slot_stride = (int)S; pub.epoch = epoch; pub.ticket = D.xticket;
+          CK(xchg_publish_launch(D.cs + off + c0, pub, D.st));
+        }
+      }
+      for (Dev &D : h->devs) {
+        CK(cudaSetDevice(D.ordinal));
+        if (rs) CK(xchg_rs_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), m, (int)S, epoch, D.cs + off + c0, D.st));
+        else CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), m, (int)S, epoch, D.cs + off + c0, D.st, op));
+      }
+    }
+    return 0;
+  }
+  if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
+  NcclApi &N = nccl_api();
+  CKN(N.GroupStart());
+  for (Dev &D : h->devs)
+    CKN(N.AllReduce(D.cs + off, D.cs + off, n, ncclDouble, op == kXchgMax ? ncclMax : ncclSum, D.comm, D.st));
+  CKN(N.GroupEnd());
+  return 0;
+}
+
+// Collective: pass 1 on every local shard, the exchange of its sums and maxima, pass 2 (mu from the exchanged sums, on the
+// device), the exchange of its sums; the host then adds a CSR column's implicit zeros in closed form.
+int agd_col_stats(agd_handle *h, double *count, double *out) {
+  if (check_ready(h)) return 1;
+  if (!count || !out) return fail(h, "NULL argument");
+  h->xg_pending = false;
+  const int32_t d = h->d, du = h->d_user;
+  const ColStatsLayout L = colstats_layout(d);
+  const size_t nsum1 = 4 * (size_t)d + 1;   // what a dense sweep's slabs carry of the pass-1 sums (STORED is filled after)
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    if (D.cs_doubles < L.total) {
+      if (D.cs) cudaFree(D.cs);
+      D.cs = nullptr;
+      D.cs_doubles = 0;
+      CK(cudaMalloc(&D.cs, L.total * sizeof(double)));
+      D.cs_doubles = L.total;
+    }
+    const Shard &s = D.sh;
+    ColStatsArgs a;
+    a.rows = s.rows; a.d = d; a.row_base = D.row_base; a.filt = h->filt_of(D); a.stream = D.st;
+    if (s.csr) {
+      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val;
+      a.out = D.cs + L.sums; a.keys = reinterpret_cast<unsigned long long *>(D.cs + L.keys);
+      CK(cudaMemsetAsync(D.cs + L.sums, 0, L.max * sizeof(double), D.st));
+      CK(cudaMemsetAsync(D.cs + L.keys, 0, 2 * (size_t)d * sizeof(double), D.st));
+      CK(colstats_csr_launch(a, 1, s.elem_bytes, D.sm_count));
+      CK(colstats_unkey_launch(a.keys, 2 * d, D.cs + L.max, D.st));
+    } else {
+      const int mb = colstats_max_blocks(D.sm_count, d);
+      if (ensure_slabs(h, D, mb, (int32_t)(nsum1 + 2 * (size_t)d))) return 1;
+      a.X = s.X; a.slabs = D.slabs; a.max_slabs = D.slabs + (size_t)mb * nsum1;
+      int blocks = 0;
+      CK(colstats_dense_launch(a, 1, s.elem_bytes, D.sm_count, &blocks));
+      CK(k1_reduce_launch(a.slabs, blocks, (int32_t)nsum1, D.cs + L.sums, nullptr, D.st));
+      CK(colstats_max_reduce_launch(a.max_slabs, blocks, 2 * d, D.cs + L.max, D.st));
+      CK(colstats_fill_stored_launch(D.cs + L.sums, d, D.st));
+    }
+  }
+  if (colstats_allreduce(h, L.sums, col_sum_n(d), kXchgSum)) return 1;
+  if (colstats_allreduce(h, L.max, 2 * (size_t)d, kXchgMax)) return 1;
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    const Shard &s = D.sh;
+    ColStatsArgs a;
+    a.rows = s.rows; a.d = d; a.row_base = D.row_base; a.filt = h->filt_of(D); a.stream = D.st; a.mu_sums = D.cs + L.sums;
+    if (s.csr) {
+      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; a.out = D.cs + L.dev; a.mu = D.cs + L.keys;   // the keys are spent
+      CK(colstats_mu_launch(D.cs + L.sums, d, D.cs + L.keys, D.st));
+      CK(cudaMemsetAsync(D.cs + L.dev, 0, 2 * (size_t)d * sizeof(double), D.st));
+      CK(colstats_csr_launch(a, 2, s.elem_bytes, D.sm_count));
+    } else {
+      a.X = s.X; a.slabs = D.slabs;
+      int blocks = 0;
+      CK(colstats_dense_launch(a, 2, s.elem_bytes, D.sm_count, &blocks));
+      CK(k1_reduce_launch(a.slabs, blocks, 2 * d, D.cs + L.dev, nullptr, D.st));
+    }
+  }
+  if (colstats_allreduce(h, L.dev, 2 * (size_t)d, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<double> r(L.keys);
+  CK(cudaMemcpyAsync(r.data(), D0.cs, L.keys * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  const double n = r[4 * (size_t)d];
+  *count = n;
+  for (int32_t c = 0; c < du; ++c) {
+    const double sum = r[c], implicit = n - r[4 * (size_t)d + 1 + c];
+    double dev = r[L.dev + c], dev2 = r[L.dev + d + c], mx = r[L.max + c], nmn = r[L.max + d + c];
+    if (implicit > 0.0) {   // CSR: the column's zeros that are not stored, each x - mu = -mu
+      const double mu = sum / n;   // the mu of pass 2
+      dev += implicit * -mu;
+      dev2 += implicit * (mu * mu);
+      mx = std::fmax(mx, 0.0);
+      nmn = std::fmax(nmn, 0.0);
+    }
+    const double v[AGD_COLSTAT_N] = {sum, r[d + c], r[2 * (size_t)d + c], r[3 * (size_t)d + c], dev, dev2, mx, -nmn};
+    for (int k = 0; k < AGD_COLSTAT_N; ++k) out[(size_t)k * du + c] = v[k];
+  }
   return 0;
 }
 

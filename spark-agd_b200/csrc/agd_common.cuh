@@ -99,8 +99,12 @@ struct XchgRs {
   unsigned long long epoch;
   unsigned int *ticket;
 };
+// The reduction the gather kernels apply to the W slots, in rank order: a sum, or a NaN-ignoring max (column maxima; a minimum
+// travels as the max of -x).  Either way every rank gets identical bits.
+enum { kXchgSum = 0, kXchgMax = 1 };
 cudaError_t xchg_rs_publish_launch(const double *acc, const XchgRs &x, cudaStream_t st);
-cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st);
+cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st,
+                                        int op = kXchgSum);
 // waits for the W finished slices and copies them to acc_out (stand-alone form of the rs gather)
 cudaError_t xchg_rs_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
                                   int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st);
@@ -110,7 +114,7 @@ inline size_t xchg_off_res(int S, int W) { return xchg_off_rs(S, W) + 2 * (size_
 inline size_t xchg_total_doubles(int S, int W) { return xchg_off_res(S, W) + 2 * (size_t)S; }
 cudaError_t xchg_publish_launch(const double *acc, const XchgPub &pub, cudaStream_t st);
 cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
-                               int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st);
+                               int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st, int op = kXchgSum);
 
 // out[c] = sum_b slabs[b][c] for c < n, n = d + 4 or 2 (d + 4) (gradient sums, loss sum, row count, loss sum and count at w2; fixed order =>
 // deterministic);
@@ -166,6 +170,38 @@ int score_max_blocks(int sm_count);
 cudaError_t score_margins_launch(const ScoreArgs &a, int elem_bytes, int sm_count);
 // *blocks_out = slabs written (0 for an empty range)
 cudaError_t score_eval_launch(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out);
+// ---------------------------------------------------------------- column statistics (colstats.cu, agd_col_stats)
+// Pass 1 sums, per device and after the exchange: [SUM d | SQ d | ABS d | NNZ d | COUNT 1 | STORED d] (col_sum_n(d) doubles);
+// maxima [MAX d | -MIN d]; pass 2 sums [DEV d | DEV2 d].  STORED is the stored-entry count of a CSR column (= COUNT on
+// dense shards), so the host adds the implicit zeros of a column, COUNT - STORED of them, in closed form.
+inline size_t col_sum_n(int32_t d) { return 5 * (size_t)d + 1; }
+struct ColStatsArgs {
+  const void *X = nullptr;          // dense shard (fp32 / fp64 / bf16), row-major, ld == d
+  const int64_t *rowptr = nullptr;  // CSR shard (fp32 / fp64 values)
+  const int32_t *idx = nullptr;
+  const void *val = nullptr;
+  int64_t rows = 0;
+  int32_t d = 0;
+  long long row_base = 0;           // global index of the shard's first row ...
+  const RowFilter *filt = nullptr;  // ... and the view whose rows are summarised (rows outside it are not read)
+  const double *mu_sums = nullptr;  // dense pass 2: the world's pass-1 sums; mu = fl(SUM / COUNT) on the device
+  const double *mu = nullptr;       // CSR pass 2: d values of mu (colstats_mu_launch)
+  double *slabs = nullptr;          // dense: [blocks][4 d + 1] (pass 1) or [blocks][2 d] (pass 2) ...
+  double *max_slabs = nullptr;      // ... and [blocks][2 d] maxima (pass 1)
+  double *out = nullptr;            // CSR: pass-1 sums (zeroed) or pass-2 sums (zeroed), scattered with RED.ADD
+  unsigned long long *keys = nullptr;   // CSR pass 1: [2 d] order-preserving images of MAX / -MIN (zeroed = none)
+  cudaStream_t stream = nullptr;
+};
+// slabs a dense sweep writes at most (its slab memory is bounded for wide rows)
+int colstats_max_blocks(int sm_count, int32_t d);
+cudaError_t colstats_dense_launch(const ColStatsArgs &a, int pass, int elem_bytes, int sm_count, int *blocks_out);
+cudaError_t colstats_csr_launch(const ColStatsArgs &a, int pass, int elem_bytes, int sm_count);
+cudaError_t colstats_unkey_launch(const unsigned long long *keys, int n, double *out, cudaStream_t st);
+cudaError_t colstats_fill_stored_launch(double *sums, int32_t d, cudaStream_t st);
+cudaError_t colstats_mu_launch(const double *sums, int32_t d, double *mu, cudaStream_t st);
+// out[c] = NaN-ignoring max over the slabs of column c < n, fixed order
+cudaError_t colstats_max_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, cudaStream_t st);
+
 // out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
 cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);
 // the same predicate as a bitmap: bit i % 32 of bits[i / 32] for rows [0, rows) (ceil(rows / 32) words)

@@ -8,6 +8,17 @@ namespace agd {
 
 namespace {
 
+// the gather's reduction over the W slots (kXchgSum / kXchgMax, agd_common.cuh), applied in rank order
+template <int OP> struct XchgOp;
+template <> struct XchgOp<kXchgSum> {
+  __device__ static double init() { return 0.0; }
+  __device__ static double apply(double s, double v) { return s + v; }
+};
+template <> struct XchgOp<kXchgMax> {
+  __device__ static double init() { return __longlong_as_double(0x7ff8000000000000LL); }   // NaN: fmax ignores it
+  __device__ static double apply(double s, double v) { return fmax(s, v); }
+};
+
 // standalone publish (the CSR path has no slab reduction to fuse it into)
 __global__ void __launch_bounds__(256) xchg_publish_kernel(const double *__restrict__ acc, const XchgPub pub) {
   __shared__ bool last;
@@ -31,7 +42,8 @@ __global__ void __launch_bounds__(256) xchg_publish_kernel(const double *__restr
   }
 }
 
-// wait for the W flags of this epoch, then add the W slots in rank order (identical bits on every rank)
+// wait for the W flags of this epoch, then add (or max) the W slots in rank order (identical bits on every rank)
+template <int OP>
 __global__ void __launch_bounds__(256) xchg_gather_kernel(const double *xbuf, const unsigned long long *flags, int world,
                                                           int buf, int n, int slot_stride, unsigned long long epoch,
                                                           double *acc_out) {
@@ -42,8 +54,8 @@ __global__ void __launch_bounds__(256) xchg_gather_kernel(const double *xbuf, co
   }
   __syncthreads();
   for (int c = blockIdx.x * 256 + threadIdx.x; c < n; c += gridDim.x * 256) {
-    double s = 0.0;
-    for (int r = 0; r < world; ++r) s += __ldcg(xbuf + ((size_t)buf * world + r) * slot_stride + c);  // written remotely: bypass L1
+    double s = XchgOp<OP>::init();
+    for (int r = 0; r < world; ++r) s = XchgOp<OP>::apply(s, __ldcg(xbuf + ((size_t)buf * world + r) * slot_stride + c));  // written remotely: bypass L1
     acc_out[c] = s;
   }
 }
@@ -75,7 +87,8 @@ __global__ void __launch_bounds__(256) xchg_rs_publish_kernel(const double *__re
   }
 }
 
-// step 2: wait for the W contributions to MY slice, add them in rank order, store the finished slice into every rank's res area
+// step 2: wait for the W contributions to MY slice, add (or max) them in rank order, store the finished slice into every rank's res area
+template <int OP>
 __global__ void __launch_bounds__(256) xchg_rs_reduce_bcast_kernel(const double *xbuf, const unsigned long long *flags, const XchgRs x) {
   __shared__ bool last;
   const int W = x.world, S = x.slot_stride;
@@ -92,8 +105,8 @@ __global__ void __launch_bounds__(256) xchg_rs_reduce_bcast_kernel(const double 
   int len = x.n - c0;
   if (len > l) len = l;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < len; i += gridDim.x * 256) {
-    double s = 0.0;
-    for (int r = 0; r < W; ++r) s += __ldcg(xbuf + off_rs + ((size_t)x.buf * W + r) * L + i);   // rank order: identical bits everywhere
+    double s = XchgOp<OP>::init();
+    for (int r = 0; r < W; ++r) s = XchgOp<OP>::apply(s, __ldcg(xbuf + off_rs + ((size_t)x.buf * W + r) * L + i));   // rank order: identical bits everywhere
     const size_t dst = off_res + (size_t)x.buf * S + (size_t)(c0 + i);
     for (int q = 0; q < W; ++q) x.peers.slot[q][dst] = s;
   }
@@ -134,12 +147,14 @@ cudaError_t xchg_rs_publish_launch(const double *acc, const XchgRs &x, cudaStrea
   xchg_rs_publish_kernel<<<grid, 256, 0, st>>>(acc, x);
   return cudaGetLastError();
 }
-cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st) {
+cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st,
+                                        int op) {
   const int l = (x.n + x.world - 1) / x.world;
   int grid = (l + 255) / 256;
   if (grid > 132) grid = 132;   // one CTA per H100 SM
   if (grid < 1) grid = 1;
-  xchg_rs_reduce_bcast_kernel<<<grid, 256, 0, st>>>(xbuf_local, flags_local, x);
+  if (op == kXchgMax) xchg_rs_reduce_bcast_kernel<kXchgMax><<<grid, 256, 0, st>>>(xbuf_local, flags_local, x);
+  else xchg_rs_reduce_bcast_kernel<kXchgSum><<<grid, 256, 0, st>>>(xbuf_local, flags_local, x);
   return cudaGetLastError();
 }
 cudaError_t xchg_rs_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
@@ -158,10 +173,11 @@ cudaError_t xchg_publish_launch(const double *acc, const XchgPub &pub, cudaStrea
 }
 
 cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
-                               int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st) {
+                               int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st, int op) {
   int grid = (n + 255) / 256;
   if (grid > 64) grid = 64;
-  xchg_gather_kernel<<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
+  if (op == kXchgMax) xchg_gather_kernel<kXchgMax><<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
+  else xchg_gather_kernel<kXchgSum><<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
   return cudaGetLastError();
 }
 
