@@ -233,6 +233,21 @@ int agd_set_row_filter(agd_handle *h, int32_t n, const uint64_t *seeds, const do
  * collective; the kernels' own predicate, so a host never restates the draw). */
 int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, uint8_t *out);
 
+/* ---- feature transforms: train on appendBias(s o x) without materialising it ----
+ * Installs the transform MLlib's GeneralizedLinearAlgorithm applies before its optimizer: each stored feature x_j is multiplied by
+ * scale[j] (StandardScaler, withMean = false: scale = 1 / sigma, or 0 where sigma = 0), and with append_bias a constant 1.0 is
+ * appended as the last feature (MLUtils.appendBias): the intercept is the last weight, regularised like every other.
+ * scale: NULL (no scaling) or agd_dim(h) finite doubles; append_bias: 0 or 1.  (NULL, 0) clears the transform.
+ * It applies to agd_smooth, agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run and agd_gd_run_minibatch: their weights and
+ * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  (agd_prox takes its dimension as an argument.)
+ * It does not apply to agd_margins, agd_evaluate, agd_col_stats, the loads or the row accessors, which address the stored
+ * features: score a transformed model there with weights s o v and intercept b.
+ * The rows are never rewritten: the gradient kernels add b to every margin and sum the multipliers for the intercept's
+ * gradient, the point is scaled (w_eff = s o v) before each sweep and the gradient columns after it, so a scaled value is never
+ * rounded to the storage type.  Like agd_set_row_filter, the transform stays until it is replaced, cleared or dropped by
+ * agd_clear, a failed install leaves none, and every rank must install the same one before a collective call. */
+int agd_set_feature_transform(agd_handle *h, const double *scale, int32_t append_bias);
+
 /* agd_prox = applyProjector (AGD.scala:214-222): Updater.compute(w, g, step, iter = 1, reg). */
 int agd_prox(agd_handle *h, int32_t updater, const double *w, const double *g, double step, double reg,
              int32_t d, double *w_out, double *reg_val);

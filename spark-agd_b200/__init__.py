@@ -11,8 +11,9 @@ from .glm import (GeneralizedLinearAlgorithm, GeneralizedLinearModel, LinearRegr
                   LogisticRegressionModel, LogisticRegressionWithAGD, SVMModel, SVMWithAGD, append_bias, column_std)
 from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
                            HingeGradient, L1Updater, LeastSquaresGradient, LogisticGradient, MLUtils, RunStats,
-                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, run_with_stats, split_bounds)
+                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, physical_model, run_with_stats, split_bounds)
 from .stat import MultivariateStatisticalSummary, Statistics
+from .feature import StandardScaler, StandardScalerModel
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -20,4 +21,5 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "GradientDescent",
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
-           "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics"]
+           "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics", "StandardScaler",
+           "StandardScalerModel", "physical_model"]

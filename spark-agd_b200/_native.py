@@ -117,6 +117,7 @@ _SIGNATURES = {
     "agd_col_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "agd_row_filter_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
+    "agd_set_feature_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "agd_prox": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_int32,
                            C.c_void_p, C.POINTER(C.c_double)]),
     "agd_run": (C.c_int, [C.c_void_p, C.POINTER(Params), C.c_void_p, C.c_void_p, C.c_void_p,

@@ -110,6 +110,9 @@ struct Dev {
   int64_t view_bits_rows = -1;     // rows the bitmap describes (-1: none) ...
   long long view_bits_base = 0;    // ... numbered from this row_base ...
   RowFilter view_bits_filt;        // ... under this filter
+  double *tf_scale = nullptr;      // the feature scaling of agd_set_feature_transform: d doubles (zero on padded columns) ...
+  double *weff = nullptr, *weff2 = nullptr;   // ... and the points K1 evaluates under it, (s o v, b) at w and at w2
+  int32_t tf_cap = 0;              // capacity of the three, in doubles
   double *hist_host = nullptr;            // pinned + mapped: [2k] = loss sum, [2k+1] = count of the history pass of iteration k
   double *hist_dev = nullptr;             // device alias of hist_host (k3_step stores the pair that rode along with a fused sweep)
   size_t hist_cap = 0;
@@ -139,6 +142,13 @@ struct agd_handle {
   unsigned long long sample_seed = 0, sample_thresh = 0;  // mini-batch row mask of the current pass (0 = every row)
   RowFilter filt;            // the view every collective sweep runs on (agd_set_row_filter; n = 0: every row) ...
   const RowFilter *filt_of(const Dev &D) const { return filt.n ? D.filt_dev : nullptr; }   // ... as the kernels get it
+  // The feature transform of agd_set_feature_transform: the model is (v, b) on appendBias(s o x).  Only K1's row loop runs in
+  // the stored width d; every vector of the solver, the payload and its offsets use the MODEL dimension model_d() = d + bias,
+  // in which the intercept is the last weight (index d internally, d_user for the caller).
+  bool tf_scale = false;
+  int32_t tf_bias = 0;
+  int32_t model_d() const { return d + tf_bias; }
+  const double *scale_of(const Dev &D) const { return tf_scale ? D.tf_scale : nullptr; }
   int collective = 0;        // 0 = auto (peer memory if every pair of ranks can map each other, else NCCL), 1 = nccl, 2 = p2p
   int32_t x_d = 0;           // dimension the exchange buffers were built for (0 = not built)
   bool x_p2p = false;        // exchange buffers are live
@@ -217,7 +227,7 @@ int free_shard(agd_handle *h, Dev &D) {
 }
 
 int ensure_vectors(agd_handle *h, Dev &D, int32_t d) {
-  if (D.vec_d == d) return 0;
+  if (D.vec_d >= d) return 0;   // a model with an intercept is one longer: switching a transform on and off reallocates nothing
   CK(cudaSetDevice(D.ordinal));
   double **v[] = {&D.x, &D.z, &D.x_old, &D.z_old, &D.y, &D.g_y, &D.g_x, &D.wtmp, &D.y_spec};
   for (double **p : v) {
@@ -233,6 +243,25 @@ int ensure_vectors(agd_handle *h, Dev &D, int32_t d) {
   CK(cudaMalloc(&D.partials, (size_t)k3_blocks(d) * K3_NS * sizeof(double)));
   D.vec_d = d;
   return 0;
+}
+
+// A point of the model (d_user + bias doubles from the caller) -> dst (model_d() doubles on the device): the features, zero
+// weights on the padded columns, the intercept last.  And back.
+int put_point(agd_handle *h, Dev &D, double *dst, const double *w) {
+  CK(cudaMemsetAsync(dst, 0, ((size_t)h->model_d() + 2) * sizeof(double), D.st));
+  CK(cudaMemcpyAsync(dst, w, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  if (h->tf_bias) CK(cudaMemcpyAsync(dst + h->d, w + h->d_user, sizeof(double), cudaMemcpyHostToDevice, D.st));
+  return 0;
+}
+int get_point(agd_handle *h, Dev &D, double *w_out, const double *src) {
+  CK(cudaMemcpyAsync(w_out, src, (size_t)h->d_user * sizeof(double), cudaMemcpyDeviceToHost, D.st));
+  if (h->tf_bias) CK(cudaMemcpyAsync(w_out + h->d_user, src + h->d, sizeof(double), cudaMemcpyDeviceToHost, D.st));
+  return 0;
+}
+// the same on host memory: the caller's d_user + bias values of a model_d() vector, divided by `div`
+void model_values(const agd_handle *h, const double *src, double div, double *out) {
+  for (int32_t j = 0; j < h->d_user; ++j) out[j] = src[j] / div;
+  if (h->tf_bias) out[h->d_user] = src[h->d] / div;
 }
 
 int ensure_slabs(agd_handle *h, Dev &D, int blocks, int32_t n) {
@@ -605,15 +634,17 @@ bool dual_full_supported(const agd_handle *h) {
 
 // One applySmooth (AGD.scala:192-208) at the device-resident point `w_of(dev)`: K1 over every local
 // shard, slab reduction, one all-reduce of [grad | loss | count | loss2 | count2].  Result: Dev::acc on every device.
-// w2_of != nullptr: the same sweep also evaluates the loss (not the gradient) at `w2_of(dev)` -> acc[d+2], acc[d+3];
-// with dual_full also the gradient there -> a second block acc[d+4 .. 2d+7] = [grad | loss | count | 0 | 0].
+// w2_of != nullptr: the same sweep also evaluates the loss (not the gradient) at `w2_of(dev)` -> acc[D+2], acc[D+3];
+// with dual_full also the gradient there -> a second block acc[D+4 .. 2D+7] = [grad | loss | count | 0 | 0].
+// D = h->model_d(): under a feature transform the points and the gradient are those of the model on appendBias(s o x);
+// K1 runs on the stored x at w_eff = (s o v, b) and the gradient columns are scaled by s before the exchange.
 // defer_gather: on the peer-memory path the gather is left to the next K3 kernel (h->xg_pending; see XchgGather) -- one launch
 // fewer per sweep; the caller must hand the pending exchange to a k3_step / k3_gx launch before anything else reads acc.
 int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = nullptr, bool dual_full = false,
                   bool defer_gather = false) {
   if (h->xg_pending) return fail(h, "internal: an exchange is still waiting for its consumer");
-  const int32_t d = h->d;
-  const int32_t n = (dual_full ? 2 : 1) * (d + 4);   // doubles this sweep produces and exchanges
+  const int32_t d = h->d, md = h->model_d();
+  const int32_t n = (dual_full ? 2 : 1) * (md + 4);   // doubles this sweep produces and exchanges
   const bool p2p = h->world > 1 && h->x_p2p;
   const bool rs = p2p && n >= kXchgRsMin;    // large payloads: reduce-scatter + all-gather instead of the one-shot exchange
   const unsigned long long epoch = p2p ? ++h->x_epoch : 0ull;
@@ -634,16 +665,28 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     CK(cudaSetDevice(D.ordinal));
     const Shard &s = D.sh;
     const bool t0 = timed && i == 0;
+    const double *w = w_of(D), *w2 = w2_of ? w2_of(D) : nullptr;
+    const double *scale = h->scale_of(D);
+    if (scale) {   // the points on the stored features: (s o v, b)
+      CK(transform_point_launch(D.weff, w, w2 ? D.weff2 : nullptr, w2, scale, d, md, D.st));
+      w = D.weff;
+      if (w2) w2 = D.weff2;
+      if (i == 0) h->launches += 1;
+    }
     if (s.csr) {
       if (dual_full) return fail(h, "internal: two-gradient sweep requested on a CSR shard");
       K1CsrArgs a;
-      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; a.labels = s.labels; a.w = w_of(D);
-      a.w2 = w2_of ? w2_of(D) : nullptr;
+      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; a.labels = s.labels; a.w = w;
+      a.w2 = w2;
       a.gacc = D.acc; a.rows = s.rows; a.d = d; a.kind = kind;
       a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.filt = h->filt_of(D); a.tune = h->tune_rows;
       if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
-      CK(k1_csr_launch(a, s.elem_bytes, D.sm_count, D.st));
+      CK(k1_csr_launch(a, h->tf_bias, s.elem_bytes, D.sm_count, D.st));
       if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
+      if (scale) {   // K1 summed the gradient straight into acc: scale it before the exchange
+        CK(scale_columns_launch(D.acc, scale, d, D.st));
+        if (i == 0) h->launches += 1;
+      }
       if (rs) {
         const XchgRs x = make_rs(D, i);
         CK(xchg_rs_publish_launch(D.acc, x, D.st));
@@ -654,7 +697,7 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     }
     if (ensure_view_bits(h, D)) return 1;
     K1Args a;
-    a.X = s.X; a.labels = s.labels; a.w = w_of(D); a.w2 = w2_of ? w2_of(D) : nullptr; a.dual_full = dual_full ? 1 : 0;
+    a.X = s.X; a.labels = s.labels; a.w = w; a.w2 = w2; a.dual_full = dual_full ? 1 : 0;
     a.rows = s.rows; a.d = d; a.kind = h->k1_diag ? h->k1_diag : kind;
     a.stages = h->ring_stages; a.slab_stride = n;
     a.sample_seed = h->sample_seed; a.sample_thresh = h->sample_thresh; a.row_base = D.row_base; a.filt = h->filt_of(D); a.view_bits = a.filt ? D.view_bits : nullptr; a.tune_rows = h->tune_rows; a.tune_ctas = h->tune_ctas; a.tune_full = h->tune_full;
@@ -678,13 +721,13 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     a.slabs = D.slabs;
     int blocks = 0;
     if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
-    if (tc) CK(k1_tc_launch(a, D.sm_count, &blocks, D.st));
-    else if (ring) CK(k1_ring_launch(a, eb, D.sm_count, &blocks, D.st));
-    else CK(k1_generic_launch(a, eb, D.sm_count, max_blocks, &blocks, D.st));
+    if (tc) CK(k1_tc_launch(a, h->tf_bias, D.sm_count, &blocks, D.st));
+    else if (ring) CK(k1_ring_launch(a, h->tf_bias, eb, D.sm_count, &blocks, D.st));
+    else CK(k1_generic_launch(a, h->tf_bias, eb, D.sm_count, max_blocks, &blocks, D.st));
     if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
     if (i == 0) trace_mark(h, dual_full ? "K1x2" : (w2_of ? "K1+loss" : "K1"));
-    if (p2p && !rs) { const XchgPub pub = make_pub(D, i); CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, &pub, D.st)); }
-    else CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, nullptr, D.st));
+    if (p2p && !rs) { const XchgPub pub = make_pub(D, i); CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, &pub, D.st, scale, d, md + 4)); }
+    else CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, nullptr, D.st, scale, d, md + 4));
     if (rs) {
       const XchgRs x = make_rs(D, i);
       CK(xchg_rs_publish_launch(D.acc, x, D.st));
@@ -769,7 +812,7 @@ int check_ready(agd_handle *h) {
   if (!h) return 1;
   if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
   for (Dev &D : h->devs)
-    if (ensure_vectors(h, D, h->d)) return 1;
+    if (ensure_vectors(h, D, h->model_d())) return 1;
   if (h->world > 1 && !h->comm_ready) return fail(h, "world_ranks=%d but agd_comm_init was not called", h->world);
   return ensure_xchg(h);
 }
@@ -903,7 +946,8 @@ int agd_destroy(agd_handle *h) {
     if (D.comm && nccl_api().ok) nccl_api().CommDestroy(D.comm);
     D.comm = nullptr;
     free_shard(h, D);
-    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval, D.cs};
+    double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval, D.cs,
+                   D.tf_scale, D.weff, D.weff2};
     for (double *p : v)
       if (p) cudaFree(p);
     if (D.ticket) cudaFree(D.ticket);
@@ -1231,6 +1275,8 @@ int agd_clear(agd_handle *h) {
   h->d = 0;
   h->d_user = 0;
   h->filt = RowFilter();
+  h->tf_scale = false;
+  h->tf_bias = 0;
   return 0;
 }
 
@@ -1349,15 +1395,11 @@ static int smooth_host(agd_handle *h, int32_t gradient, const double *w, const d
   if (!w || !loss || !grad) return fail(h, "NULL argument");
   if (w2 && !dual_supported(h)) return fail(h, "this shard's gradient kernel has no two-point form (use two agd_smooth calls)");
   if (grad2 && !dual_full_supported(h)) return fail(h, "this shard's gradient kernel has no two-gradient form (use two agd_smooth calls)");
-  const int32_t d = h->d;
+  const int32_t d = h->model_d();
   for (Dev &D : h->devs) {
     CK(cudaSetDevice(D.ordinal));
-    CK(cudaMemsetAsync(D.wtmp, 0, ((size_t)d + 2) * sizeof(double), D.st));                            // zero weights on padded columns
-    CK(cudaMemcpyAsync(D.wtmp, w, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));  // = broadcast, AGD.scala:193
-    if (w2) {
-      CK(cudaMemsetAsync(D.g_x, 0, ((size_t)d + 2) * sizeof(double), D.st));   // g_x doubles as the staging vector of w2
-      CK(cudaMemcpyAsync(D.g_x, w2, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));
-    }
+    if (put_point(h, D, D.wtmp, w)) return 1;                  // = broadcast, AGD.scala:193
+    if (w2 && put_point(h, D, D.g_x, w2)) return 1;            // g_x doubles as the staging vector of w2
   }
   h->devs[0].ev_used = h->devs[0].ev_ar_used = 0;
   h->launches = h->collectives = 0;
@@ -1372,12 +1414,12 @@ static int smooth_host(agd_handle *h, int32_t gradient, const double *w, const d
   for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
   const double cnt = host[(size_t)d + 1];
   *loss = host[d] / cnt;                                    // AGD.scala:207
-  for (int32_t j = 0; j < h->d_user; ++j) grad[j] = host[j] / cnt;
+  model_values(h, host.data(), cnt, grad);
   if (count) *count = (int64_t)cnt;
   if (w2 && loss2) *loss2 = host[(size_t)d + 2] / host[(size_t)d + 3];
   if (grad2) {  // second block: [grad at w2 | loss | count | 0 | 0]
     const double *b2 = host.data() + (size_t)d + 4;
-    for (int32_t j = 0; j < h->d_user; ++j) grad2[j] = b2[j] / b2[(size_t)d + 1];
+    model_values(h, b2, b2[(size_t)d + 1], grad2);
   }
   return 0;
 }
@@ -1426,7 +1468,7 @@ int agd_margins(agd_handle *h, int32_t dev, const double *w, double intercept, i
                 (long long)rows, (long long)s.rows, dev);
   if (!w || (rows > 0 && !out)) return fail(h, "NULL argument");
   if (rows == 0) return 0;
-  if (ensure_vectors(h, D, h->d)) return 1;
+  if (ensure_vectors(h, D, h->model_d())) return 1;
   CK(cudaSetDevice(D.ordinal));
   if (stage_weights(h, D, w)) return 1;
   // margins depend on the row only, so the range is scored in chunks through the staging buffer
@@ -1692,6 +1734,43 @@ int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, 
   return 0;
 }
 
+// ---------------------------------------------------------------- feature transforms (scaling, intercept)
+int agd_set_feature_transform(agd_handle *h, const double *scale, int32_t append_bias) {
+  if (!h) return 1;
+  if (append_bias != 0 && append_bias != 1) return fail(h, "append_bias must be 0 or 1 (got %d)", append_bias);
+  // Until every device holds the new transform the handle runs without one: a failure part-way leaves none installed.
+  h->tf_scale = false;
+  h->tf_bias = 0;
+  if (!scale && !append_bias) return 0;
+  if (h->d <= 0) return fail(h, "no shard loaded: a feature transform is sized by the feature dimension");
+  std::vector<double> s((size_t)h->d, 0.0);   // zero on the padded columns
+  if (scale)
+    for (int32_t j = 0; j < h->d_user; ++j) {
+      if (!std::isfinite(scale[j])) return fail(h, "scale[%d] = %g is not finite", j, scale[j]);
+      s[(size_t)j] = scale[j];
+    }
+  const int32_t cap = h->d + 5;   // model_d() + 4 with an intercept
+  for (Dev &D : h->devs) {   // stream-ordered after every sweep that still reads the previous transform
+    CK(cudaSetDevice(D.ordinal));
+    if (D.tf_cap < cap) {
+      CK(cudaStreamSynchronize(D.st));
+      double **bufs[] = {&D.tf_scale, &D.weff, &D.weff2};
+      for (double **b : bufs) {
+        if (*b) cudaFree(*b);
+        *b = nullptr;
+      }
+      D.tf_cap = 0;
+      for (double **b : bufs) CK(cudaMalloc(b, (size_t)cap * sizeof(double)));
+      D.tf_cap = cap;
+    }
+    if (scale) CK(cudaMemcpyAsync(D.tf_scale, s.data(), s.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
+    CK(cudaStreamSynchronize(D.st));
+  }
+  h->tf_scale = scale != nullptr;
+  h->tf_bias = append_bias;
+  return 0;
+}
+
 // ---------------------------------------------------------------- applyProjector with host buffers
 int agd_prox(agd_handle *h, int32_t updater, const double *w, const double *g, double step, double reg,
              int32_t d, double *w_out, double *reg_val) {
@@ -1726,8 +1805,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
   if (p->gradient < 0 || p->gradient > AGD_GRAD_LEAST_SQUARES_HALF) return fail(h, "unknown gradient %d", p->gradient);
   if (p->updater < 0 || p->updater > AGD_UPD_L1) return fail(h, "unknown updater %d", p->updater);
   const auto t_begin = std::chrono::steady_clock::now();
-  const int32_t d = h->d;
-  const size_t vb = (size_t)d * sizeof(double);
+  const int32_t d = h->model_d();
   const double INF = std::numeric_limits<double>::infinity();
   agd_stats s;
   memset(&s, 0, sizeof s);
@@ -1749,8 +1827,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
 
   for (Dev &D : h->devs) {                                                 // :224-225  x = w0 ; z = x
     CK(cudaSetDevice(D.ordinal));
-    CK(cudaMemsetAsync(D.x, 0, vb, D.st));  // padded columns carry zero weights throughout
-    CK(cudaMemcpyAsync(D.x, w0, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));
+    if (put_point(h, D, D.x, w0)) return 1;  // padded columns carry zero weights throughout
     CK(k3_copy2_launch(D.z, D.x, nullptr, nullptr, d, D.st));
   }
   h->launches += 1;
@@ -1791,7 +1868,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
   auto take_gather = [&](Dev &D) {
     XchgGather g;
     if (h->xg_pending) {
-      const int S = xchg_slot_stride(d), W = h->world;
+      const int S = xchg_slot_stride(h->d), W = h->world;
       g.world = W; g.buf = (int)(h->xg_epoch & 1ull); g.n = h->xg_n; g.slot_stride = S; g.epoch = h->xg_epoch;
       g.rs = h->xg_rs ? 1 : 0;
       g.xbuf = h->xg_rs ? D.xbuf + xchg_off_res(S, W) : D.xbuf;       // rs: the area of finished sums
@@ -1963,7 +2040,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
   {
     Dev &D = h->devs[0];
     CK(cudaSetDevice(D.ordinal));
-    CK(cudaMemcpyAsync(w_out, D.x, (size_t)h->d_user * sizeof(double), cudaMemcpyDeviceToHost, D.st));    // :337
+    if (get_point(h, D, w_out, D.x)) return 1;                             // :337
   }
   if (h->xg_pending || pending_hist >= 0) return fail(h, "internal: a sweep was left without its consumer");
   if (call_end(h, s, t_begin)) return 1;
@@ -1993,7 +2070,7 @@ int agd_gd_run_minibatch(agd_handle *h, int32_t gradient, int32_t updater, doubl
   if (gradient < 0 || gradient > AGD_GRAD_LEAST_SQUARES_HALF) return fail(h, "unknown gradient %d", gradient);
   if (updater < 0 || updater > AGD_UPD_L1) return fail(h, "unknown updater %d", updater);
   const auto t_begin = std::chrono::steady_clock::now();
-  const int32_t d = h->d;
+  const int32_t d = h->model_d();
   const size_t vb = (size_t)d * sizeof(double);
   agd_stats s;
   memset(&s, 0, sizeof s);
@@ -2017,8 +2094,7 @@ int agd_gd_run_minibatch(agd_handle *h, int32_t gradient, int32_t updater, doubl
   };
   for (Dev &D : h->devs) {
     CK(cudaSetDevice(D.ordinal));
-    CK(cudaMemsetAsync(D.x, 0, vb, D.st));  // padded columns carry zero weights throughout
-    CK(cudaMemcpyAsync(D.x, w0, (size_t)h->d_user * sizeof(double), cudaMemcpyHostToDevice, D.st));
+    if (put_point(h, D, D.x, w0)) return 1;  // padded columns carry zero weights throughout
     CK(cudaMemsetAsync(D.g_x, 0, vb, D.st));
   }
   // regVal = updater.compute(weights, zeros, 0, 1, regParam)._2
@@ -2045,7 +2121,7 @@ int agd_gd_run_minibatch(agd_handle *h, int32_t gradient, int32_t updater, doubl
   {
     Dev &D = h->devs[0];
     CK(cudaSetDevice(D.ordinal));
-    CK(cudaMemcpyAsync(w_out, D.x, (size_t)h->d_user * sizeof(double), cudaMemcpyDeviceToHost, D.st));
+    if (get_point(h, D, w_out, D.x)) return 1;
   }
   if (call_end(h, s, t_begin)) return 1;
   *n_hist = nh;

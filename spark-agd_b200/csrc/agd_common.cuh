@@ -45,17 +45,20 @@ struct K1Args {
   int32_t tc_margins_f64; // wgmma kernel: 1 = fp64-exact margins on the CUDA cores (option tc_margins=f64), 0 = fp32 (default)
 };
 
-// launch helpers (k1_dense.cu); return the number of blocks that wrote a slab
+// launch helpers (k1_dense.cu); return the number of blocks that wrote a slab.
+// bias = 1: the model has an intercept, w[d] (and w2[d]), and every payload block is [grad (d) | sum of the multipliers | loss |
+// count | loss2 | count2], D + 4 doubles with D = d + 1 (slab_stride and the slabs sized for it).  It is an argument of the
+// launch, not a field of K1Args: the kernels without an intercept keep the parent's parameter block, registers and bits.
 int k1_ring_supported(int32_t d, int elem_bytes);
 int k1_ring_dual_supported(int32_t d, int elem_bytes);
-cudaError_t k1_ring_launch(const K1Args &a, int elem_bytes, int sm_count, int *blocks_out, cudaStream_t st);
+cudaError_t k1_ring_launch(const K1Args &a, int bias, int elem_bytes, int sm_count, int *blocks_out, cudaStream_t st);
 int k1_ring_dual_full_supported(int32_t d, int elem_bytes);
-cudaError_t k1_generic_launch(const K1Args &a, int elem_bytes, int sm_count, int max_blocks, int *blocks_out,
+cudaError_t k1_generic_launch(const K1Args &a, int bias, int elem_bytes, int sm_count, int max_blocks, int *blocks_out,
                               cudaStream_t st);
 int k1_max_blocks(int sm_count);
 // bf16 shards: margins on CUDA cores, X^T r on wgmma (k1_tc.cu); d % 128 == 0, d <= 4096
 int k1_tc_supported(int32_t d, int elem_bytes);
-cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStream_t st);
+cudaError_t k1_tc_launch(const K1Args &a, int bias, int sm_count, int *blocks_out, cudaStream_t st);
 // ---------------------------------------------------------------- K2': one-shot all-reduce over NVLink peer memory
 // Every rank owns an exchange buffer xbuf[2][W][n] (+ flags[2][W]) that all peers can store into (P2P / CUDA IPC).
 // publish: rank r stores its n = d+4 partial sums into slot r of EVERY rank's buffer, fences, then raises the flag
@@ -116,10 +119,18 @@ cudaError_t xchg_publish_launch(const double *acc, const XchgPub &pub, cudaStrea
 cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
                                int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st, int op = kXchgSum);
 
-// out[c] = sum_b slabs[b][c] for c < n, n = d + 4 or 2 (d + 4) (gradient sums, loss sum, row count, loss sum and count at w2; fixed order =>
+// out[c] = sum_b slabs[b][c] for c < n, n = D + 4 or 2 (D + 4) (gradient sums, loss sum, row count, loss sum and count at w2; fixed order =>
 // deterministic);
-// with pub != nullptr the sums are also stored into every peer's exchange slot and the epoch flag is raised
-cudaError_t k1_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, const XchgPub *pub, cudaStream_t st);
+// with pub != nullptr the sums are also stored into every peer's exchange slot and the epoch flag is raised;
+// with scale != nullptr column c % blk < scale_d is multiplied by scale[c % blk] first (feature scaling, blk = D + 4)
+cudaError_t k1_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, const XchgPub *pub, cudaStream_t st,
+                             const double *scale = nullptr, int32_t scale_d = 0, int32_t blk = 1);
+// Feature scaling around K1 (agd_set_feature_transform).  out[c] = s[c] w[c] for c < d, w[c] for d <= c < n (the intercept);
+// the same from w2 into out2 unless out2 is null
+cudaError_t transform_point_launch(double *out, const double *w, double *out2, const double *w2, const double *s, int32_t d,
+                                   int32_t n, cudaStream_t st);
+// acc[c] *= s[c], c < d (the CSR gradient, which K1 sums straight into acc)
+cudaError_t scale_columns_launch(double *acc, const double *s, int32_t d, cudaStream_t st);
 
 // CSR variant (k1_csr.cu)
 struct K1CsrArgs {
@@ -129,7 +140,7 @@ struct K1CsrArgs {
   const double *labels;
   const double *w;
   const double *w2;       // optional second point (loss only), as in K1Args
-  double *gacc;           // d + 4 doubles, zeroed by the launch: gradient sum, loss sum, count; loss sum, count at w2
+  double *gacc;           // d + 4 doubles (d + 5 with bias), zeroed by the launch: gradient sum, loss sum, count; loss sum, count at w2
   int64_t rows;
   int32_t d;
   int32_t kind;
@@ -138,12 +149,13 @@ struct K1CsrArgs {
   const RowFilter *filt;  // as in K1Args
   int32_t tune;           // option ring_rows: 1 = the simple (unpipelined) loop
 };
-cudaError_t k1_csr_launch(const K1CsrArgs &a, int elem_bytes, int sm_count, cudaStream_t st);
+cudaError_t k1_csr_launch(const K1CsrArgs &a, int bias, int elem_bytes, int sm_count, cudaStream_t st);
 
 // Slot stride of the peer-memory exchange (doubles per rank's slot): the largest payload any sweep on a handle of this
-// dimension publishes -- 2 (d + 4) for a two-gradient sweep, AGD_EVAL_N for an evaluation.  ONE stride per handle: sweeps
-// of different payloads must not move the slots of the other parity buffer.
-inline int xchg_slot_stride(int32_t d) { return 2 * (d + 4) > AGD_EVAL_N ? 2 * (d + 4) : AGD_EVAL_N; }
+// dimension publishes -- 2 (d + 5) for a two-gradient sweep with an intercept, AGD_EVAL_N for an evaluation.  ONE stride per
+// handle, whether or not a transform is installed: sweeps of different payloads must not move the slots of the other parity
+// buffer, and the host-shipped (ipc) exchange is built once per dimension.
+inline int xchg_slot_stride(int32_t d) { return 2 * (d + 5) > AGD_EVAL_N ? 2 * (d + 5) : AGD_EVAL_N; }
 
 // ---------------------------------------------------------------- scoring sweeps (score.cu)
 // Margins m_i = x_i . w + b of rows [row0, row0 + rows) of one shard, or the AGD_EVAL_* sums over them (one slab of

@@ -150,7 +150,9 @@ __device__ __forceinline__ double warp_rows_reduce_perm(double (&p)[R]) {
 // ---------------------------------------------------------------- the hot kernel
 // VIEW: the launch runs on a view (a.filt != nullptr).  Launches without one take the instantiation that has no view code at
 // all, so their registers and instructions are those of a kernel that never heard of views.
-template <typename T, int NT, int TPR, int V, int R, int MINB, int MODE, bool VIEW>
+// BIAS: the model has an intercept (the launch's bias argument): w[d] (w2[d]) is added to every margin at w (w2), and the multipliers of the kept
+// rows are summed into slot d of the slab, so the scalar slots start at d + 1.  BIAS = false is the kernel without it.
+template <typename T, int NT, int TPR, int V, int R, int MINB, int MODE, bool VIEW, bool BIAS>
 __global__ void __launch_bounds__(NT, MINB)
 k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uint32_t aux_bytes) {
   constexpr int EPV = Elem<T>::EPV;
@@ -208,6 +210,10 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
     }
     mbar_init(wbar, 1);
     mbar_fence_init();
+    // BIAS: red[lane] sums the multipliers of the rows lane `lane` of the scalar warps evaluates (the rotating scalar warps
+    // take turns between CTA barriers); red is only used after the row loop otherwise
+    if (BIAS)
+      for (int l = 0; l < 32; ++l) red[l] = 0.0;
     mbar_expect_tx(wbar, (uint32_t)a.d * 8u * NP);
     tma_bulk_g2s(smem_u32(aux), a.w, (uint32_t)a.d * 8u, wbar);  // w: TMA-staged once per CTA
     if (DUAL) tma_bulk_g2s(smem_u32(aux + kPointBytes), a.w2, (uint32_t)a.d * 8u, wbar);
@@ -410,7 +416,8 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
       double pw[8];
 #pragma unroll
       for (int wi = 0; wi < 8; ++wi) pw[wi] = (wi < WPG) ? pp[srow * 8 + wi] : 0.0;
-      const double m = ((pw[0] + pw[1]) + (pw[2] + pw[3])) + ((pw[4] + pw[5]) + (pw[6] + pw[7]));
+      double m = ((pw[0] + pw[1]) + (pw[2] + pw[3])) + ((pw[4] + pw[5]) + (pw[6] + pw[7]));
+      if (BIAS) m += ld_volatile_f64((DUAL && lane >= 16) ? a.w2 + a.d : a.w + a.d);
       // VIEW: the row's bit of the view bitmap (row_in_view() of every row, drawn once when the filter was set) -- one load,
       // where the Philox rounds of row_in_view() would need registers this section does not have
       row_ok = srow < rv && (!VIEW || ((a.view_bits[(row0 + srow) >> 5] >> ((row0 + srow) & 31)) & 1u) != 0u) &&
@@ -423,6 +430,7 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
       if (MODE == 2 && lane >= 16) mult2_s[srow] = mw;
       if (a.kind != AGD_GRAD_LOGISTIC) lossacc += row_ok ? loss : 0.0;
       cntacc += row_ok ? 1.0 : 0.0;
+      if (BIAS) red[lane] += mw;
       // A row whose multiplier is exactly 0 adds nothing (netlib DAXPY returns when DA == 0), but 0 * inf is NaN.  Flag the
       // rows where that can happen: a finite margin means every feature of the row is finite (padded columns are zero).
       // Bit = tile row; with a second gradient (MODE 2), bits 16 + row are the rows at w2.
@@ -485,7 +493,9 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
   }
 
   // ---------------- per-CTA slab: column sums (row groups added in fixed order) and loss sum.  MODE 2: a second block of
-  // d + 4 doubles [gradient at w2 | loss sum | count | 0 | 0] follows the first.
+  // D + 4 doubles [gradient at w2 | loss sum | count | 0 | 0] follows the first (D = d + BIAS: with BIAS the gradient ends
+  // in the multiplier sum).
+  const int DB = a.d + (BIAS ? 1 : 0);
   double *slab = a.slabs + (size_t)blockIdx.x * a.slab_stride;
   auto write_columns = [&](double (&av)[V][EPV], double *dst) {
     if (NG > 1) {
@@ -519,12 +529,22 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
     }
   };
   write_columns(acc, slab);
-  if (MODE == 2) write_columns(reinterpret_cast<double (&)[V][EPV]>(accB), slab + a.d + 4);
+  if (MODE == 2) write_columns(reinterpret_cast<double (&)[V][EPV]>(accB), slab + DB + 4);
   // DUAL: lanes 16-31 hold the sums at w2.  Skipping the xor-16 step leaves the lane-0 total bit-identical to the
   // single-point kernel's, whose lanes >= 16 only ever contribute exact zeros.
   for (int off = DUAL ? 8 : 16; off >= 1; off >>= 1) {
     lossacc += __shfl_xor_sync(0xffffffffu, lossacc, off);
     cntacc += __shfl_xor_sync(0xffffffffu, cntacc, off);
+  }
+  if (BIAS) {   // the multiplier sums leave red for `partial` (free since the last tile's barrier) before red takes the loss sums
+    __syncthreads();
+    if (warp == 0) {
+      double macc = red[lane];
+      for (int off = DUAL ? 8 : 16; off >= 1; off >>= 1) macc += __shfl_xor_sync(0xffffffffu, macc, off);
+      if (lane == 0) partial[0] = macc;
+      if (MODE == 2 && lane == 16) partial[1] = macc;
+    }
+    __syncthreads();
   }
   if (lane == 0) { red[warp] = lossacc; red[8 + warp] = cntacc; }
   if (DUAL && lane == 16) { red[16 + warp] = lossacc; red[24 + warp] = cntacc; }
@@ -534,16 +554,20 @@ k1_ring_kernel(const K1Args a, const int nvec, const long long ntiles, const uin
     for (int wi = 0; wi < NW; ++wi) { sacc += red[wi]; cacc += red[8 + wi]; }
     if (DUAL)
       for (int wi = 0; wi < NW; ++wi) { sacc2 += red[16 + wi]; cacc2 += red[24 + wi]; }
-    slab[a.d] = sacc;
-    slab[a.d + 1] = cacc;
-    slab[a.d + 2] = sacc2;   // loss sum and row count at w2 (zero when the launch has no second point)
-    slab[a.d + 3] = cacc2;
+    if (BIAS) {
+      slab[a.d] = partial[0];
+      if (MODE == 2) slab[DB + 4 + a.d] = partial[1];
+    }
+    slab[DB] = sacc;
+    slab[DB + 1] = cacc;
+    slab[DB + 2] = sacc2;   // loss sum and row count at w2 (zero when the launch has no second point)
+    slab[DB + 3] = cacc2;
     if (MODE == 2) {
-      double *slab2 = slab + a.d + 4;
-      slab2[a.d] = sacc2;
-      slab2[a.d + 1] = cacc2;
-      slab2[a.d + 2] = 0.0;
-      slab2[a.d + 3] = 0.0;
+      double *slab2 = slab + DB + 4;
+      slab2[DB] = sacc2;
+      slab2[DB + 1] = cacc2;
+      slab2[DB + 2] = 0.0;
+      slab2[DB + 3] = 0.0;
     }
   }
 }
@@ -556,7 +580,8 @@ template <> __device__ __forceinline__ double load_elem<__nv_bfloat16>(const __n
 // ---------------------------------------------------------------- generic shapes
 // a.w2 != nullptr: the loss (not the gradient) is also evaluated at w2 in the same sweep -- threads 32..32+R-1 play the
 // part of threads 0..R-1 for it, so its sum is formed exactly as a launch of its own would form it.
-template <typename T, bool VIEW>
+// BIAS: as in the ring kernel (w[d] / w2[d] on the margins, the multiplier sum in slot d, scalars from d + 1)
+template <typename T, bool VIEW, bool BIAS>
 __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const long long ntiles) {
   constexpr int R = 8;
   __shared__ double part[2][R][8];
@@ -567,7 +592,7 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
   const T *X = reinterpret_cast<const T *>(a.X);
   double *slab = a.slabs + (size_t)blockIdx.x * a.slab_stride;
   for (int c = tid; c <= a.d; c += 256) slab[c] = 0.0;
-  double lossacc = 0.0, cntacc = 0.0;
+  double lossacc = 0.0, cntacc = 0.0, multacc = 0.0;
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long row0 = tile * R;
     const long long left = a.rows - row0;
@@ -606,12 +631,14 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
       double m = 0.0;
 #pragma unroll
       for (int wi = 0; wi < 8; ++wi) m += part[which][srow][wi];
+      if (BIAS) m += (which ? a.w2 : a.w)[a.d];
       double mult = 0.0, loss = 0.0;
       if (srow < rv && row_kept(a.sample_seed, a.sample_thresh, VIEW ? a.filt : nullptr, a.row_base + row0 + srow)) {
         loss_eval(a.kind, m, a.labels[row0 + srow], mult, loss);
         cntacc += 1.0;
       }
       if (which == 0) mult_s[srow] = mult;
+      if (BIAS && which == 0) multacc += mult;
       lossacc += loss;
     }
     __syncthreads();
@@ -631,21 +658,24 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
   for (int off = 16; off >= 1; off >>= 1) {
     lossacc += __shfl_xor_sync(0xffffffffu, lossacc, off);
     cntacc += __shfl_xor_sync(0xffffffffu, cntacc, off);
+    if (BIAS) multacc += __shfl_xor_sync(0xffffffffu, multacc, off);
   }
-  if (lane == 0) { red[warp] = lossacc; red[8 + warp] = cntacc; }
+  if (lane == 0) { red[warp] = lossacc; red[8 + warp] = cntacc; if (BIAS) red[16 + warp] = multacc; }
   __syncthreads();
   if (tid == 0) {
     // warp 0 carries the sums at w, warp 1 those at w2 (all other entries are exact zeros)
+    const int DB = a.d + (BIAS ? 1 : 0);
     double sacc = 0.0, cacc = 0.0, sacc2 = 0.0, cacc2 = 0.0;
     for (int wi = 0; wi < 8; ++wi) {
       if (dual && wi == 1) { sacc2 = red[wi]; cacc2 = red[8 + wi]; continue; }
       sacc += red[wi];
       cacc += red[8 + wi];
     }
-    slab[a.d] = sacc;
-    slab[a.d + 1] = cacc;
-    slab[a.d + 2] = sacc2;
-    slab[a.d + 3] = cacc2;
+    if (BIAS) slab[a.d] = red[16];   // only warp 0 evaluates rows at w
+    slab[DB] = sacc;
+    slab[DB + 1] = cacc;
+    slab[DB + 2] = sacc2;
+    slab[DB + 3] = cacc2;
   }
 }
 
@@ -654,9 +684,13 @@ __global__ void __launch_bounds__(256) k1_generic_kernel(const K1Args a, const l
 // fused sweep; after a two-gradient sweep a second such block).  32 columns per block; 8 slab groups per block sum
 // strided subsets (slab b -> group b % 8) with 4 loads in flight, then group 0 adds the 8 group sums in
 // order: the summation tree is fixed, so the result is bit-reproducible.
-template <bool PUB>
+// SCALE: the gradient columns c < sd of every block of blk doubles are multiplied by scale[c] before they are stored and
+// published (the feature scaling of agd_set_feature_transform: d/dv_j of x (s o v) is s_j sum_i r_i x_ij).  Each rank scales
+// its own partial, so the rank-ordered sum of the exchange still gives every rank the same bits.
+template <bool PUB, bool SCALE>
 __global__ void __launch_bounds__(256) k1_reduce_kernel(const double *__restrict__ slabs, int blocks, int n,
-                                                        double *__restrict__ out, const XchgPub pub) {
+                                                        double *__restrict__ out, const XchgPub pub,
+                                                        const double *__restrict__ scale, int sd, int blk) {
   __shared__ double part[8][33];
   __shared__ bool last;
   const int cl = threadIdx.x & 31, grp = threadIdx.x >> 5;
@@ -678,6 +712,7 @@ __global__ void __launch_bounds__(256) k1_reduce_kernel(const double *__restrict
     double t = 0.0;
 #pragma unroll
     for (int gi = 0; gi < 8; ++gi) t += part[gi][cl];
+    if (SCALE) { const int cc = c % blk; if (cc < sd) t *= scale[cc]; }
     out[c] = t;
     if (PUB) {  // compute + collective in one kernel: the result goes straight into every peer's HBM over NVLink
       const size_t off = ((size_t)pub.buf * pub.world + pub.my_rank) * pub.slot_stride + c;
@@ -734,7 +769,7 @@ inline bool ring_shape(int32_t d, int elem_bytes, RingShape &sh, int &nvec) {
 }
 
 template <typename T, int NT, int TPR, int V, int R, int MINB, int MODE = 0>
-cudaError_t launch_ring_inst(const K1Args &a_in, int nvec, int sm_count, int *blocks_out, cudaStream_t st) {
+cudaError_t launch_ring_inst(const K1Args &a_in, int bias, int nvec, int sm_count, int *blocks_out, cudaStream_t st) {
   constexpr int EPV = Elem<T>::EPV;
   constexpr int NG = NT / TPR;
   constexpr int TR = NG * R;
@@ -751,19 +786,22 @@ cudaError_t launch_ring_inst(const K1Args &a_in, int nvec, int sm_count, int *bl
   int stages = a.stages > 0 ? a.stages : 4;
   while (stages > 1 && ring_layout(tile_bytes, aux_bytes, stages, MODE).total > budget) --stages;
   a.stages = stages;
-  a.slab_stride = (MODE == 2 ? 2 : 1) * (a.d + 4);
+  a.slab_stride = (MODE == 2 ? 2 : 1) * (a.d + bias + 4);
   const RingLayout L = ring_layout(tile_bytes, aux_bytes, stages, MODE);
-  const int view = a.filt ? 1 : 0;
-  auto kern = view ? k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, true> : k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, false>;
+  const int view = a.filt ? 1 : 0, form = view + 2 * (bias ? 1 : 0);
+  auto kern = bias ? (view ? k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, true, true>
+                             : k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, false, true>)
+                     : (view ? k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, true, false>
+                             : k1_ring_kernel<T, NT, TPR, V, R, MINB, MODE, false, false>);
   // the opt-in shared-memory size is a per-device property of the function: set it when it changes, not on every launch
-  static int smem_set[2][64] = {};
+  static int smem_set[4][64] = {};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64 || smem_set[view][dev] != (int)L.total) {
+  if (dev < 0 || dev >= 64 || smem_set[form][dev] != (int)L.total) {
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) smem_set[view][dev] = (int)L.total;
+    if (dev >= 0 && dev < 64) smem_set[form][dev] = (int)L.total;
   }
   const long long ntiles = (a.rows + TR - 1) / TR;
   long long grid = (long long)MINB * sm_count;
@@ -774,67 +812,67 @@ cudaError_t launch_ring_inst(const K1Args &a_in, int nvec, int sm_count, int *bl
   return cudaGetLastError();
 }
 
-cudaError_t launch_ring_bf16(const K1Args &a, const RingShape &sh, int nvec, int sm_count, int *blocks_out,
+cudaError_t launch_ring_bf16(const K1Args &a, int bias, const RingShape &sh, int nvec, int sm_count, int *blocks_out,
                              cudaStream_t st) {
   using T = __nv_bfloat16;
   if (a.w2 && a.dual_full) return cudaErrorInvalidValue;  // the two-gradient sweep exists for fp32 / fp64 storage
   if (a.w2) {  // fused sweep: tiles of at most 16 rows
-    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 2, 2, 1>(a, nvec, sm_count, blocks_out, st);
+    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 2, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
     switch (sh.tpr) {
-      case 64: return launch_ring_inst<T, 256, 64, 1, 4, 2, 1>(a, nvec, sm_count, blocks_out, st);
-      case 128: return launch_ring_inst<T, 256, 128, 1, 4, 2, 1>(a, nvec, sm_count, blocks_out, st);
-      case 256: return launch_ring_inst<T, 256, 256, 1, 4, 2, 1>(a, nvec, sm_count, blocks_out, st);
+      case 64: return launch_ring_inst<T, 256, 64, 1, 4, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
+      case 128: return launch_ring_inst<T, 256, 128, 1, 4, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
+      case 256: return launch_ring_inst<T, 256, 256, 1, 4, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
       default: return cudaErrorInvalidValue;
     }
   }
-  if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 2, 2>(a, nvec, sm_count, blocks_out, st);
+  if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 2, 2>(a, bias, nvec, sm_count, blocks_out, st);
   switch (sh.tpr) {
-    case 32: return launch_ring_inst<T, 256, 32, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
-    case 64: return launch_ring_inst<T, 256, 64, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
-    case 128: return launch_ring_inst<T, 256, 128, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
-    default: return launch_ring_inst<T, 256, 256, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
+    case 32: return launch_ring_inst<T, 256, 32, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+    case 64: return launch_ring_inst<T, 256, 64, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+    case 128: return launch_ring_inst<T, 256, 128, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+    default: return launch_ring_inst<T, 256, 256, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
   }
 }
 
 template <typename T>
-cudaError_t launch_ring_t(const K1Args &a, const RingShape &sh, int nvec, int sm_count, int *blocks_out,
+cudaError_t launch_ring_t(const K1Args &a, int bias, const RingShape &sh, int nvec, int sm_count, int *blocks_out,
                           cudaStream_t st) {
   if (a.w2 && a.dual_full) {  // two full evaluations per sweep (speculative sweep of the memoised pass structure)
     if (sh.v == 4) return cudaErrorInvalidValue;   // four vectors per thread: no registers for a second gradient
-    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2, 2>(a, nvec, sm_count, blocks_out, st);
-    if (sh.tpr == 128) return launch_ring_inst<T, 256, 128, 1, 8, 2, 2>(a, nvec, sm_count, blocks_out, st);
-    if (sh.tpr == 256) return launch_ring_inst<T, 256, 256, 1, 8, 2, 2>(a, nvec, sm_count, blocks_out, st);
+    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2, 2>(a, bias, nvec, sm_count, blocks_out, st);
+    if (sh.tpr == 128) return launch_ring_inst<T, 256, 128, 1, 8, 2, 2>(a, bias, nvec, sm_count, blocks_out, st);
+    if (sh.tpr == 256) return launch_ring_inst<T, 256, 256, 1, 8, 2, 2>(a, bias, nvec, sm_count, blocks_out, st);
     return cudaErrorInvalidValue;
   }
   if (a.w2) {  // fused sweep: tiles of at most 16 rows
-    if (sh.v == 4) return launch_ring_inst<T, 256, 256, 4, 2, 2, 1>(a, nvec, sm_count, blocks_out, st);
-    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2, 1>(a, nvec, sm_count, blocks_out, st);
-    if (sh.tpr == 128) return launch_ring_inst<T, 256, 128, 1, 8, 2, 1>(a, nvec, sm_count, blocks_out, st);
-    if (sh.tpr == 256) return launch_ring_inst<T, 256, 256, 1, 8, 2, 1>(a, nvec, sm_count, blocks_out, st);
+    if (sh.v == 4) return launch_ring_inst<T, 256, 256, 4, 2, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
+    if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
+    if (sh.tpr == 128) return launch_ring_inst<T, 256, 128, 1, 8, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
+    if (sh.tpr == 256) return launch_ring_inst<T, 256, 256, 1, 8, 2, 1>(a, bias, nvec, sm_count, blocks_out, st);
     return cudaErrorInvalidValue;
   }
   if (sh.v == 1) {
     switch (sh.tpr) {
-      case 32: return launch_ring_inst<T, 256, 32, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
-      case 64: return launch_ring_inst<T, 256, 64, 1, 8, 2>(a, nvec, sm_count, blocks_out, st);
-      case 128: return launch_ring_inst<T, 256, 128, 1, 8, 2>(a, nvec, sm_count, blocks_out, st);
+      case 32: return launch_ring_inst<T, 256, 32, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+      case 64: return launch_ring_inst<T, 256, 64, 1, 8, 2>(a, bias, nvec, sm_count, blocks_out, st);
+      case 128: return launch_ring_inst<T, 256, 128, 1, 8, 2>(a, bias, nvec, sm_count, blocks_out, st);
       default: {
         // tuning variants of the headline shape: (threads per CTA) x (rows per tile) x (resident CTAs per SM)
         const int key = a.tune_rows * 10 + a.tune_ctas;
         switch (key) {
-          case 81: return launch_ring_inst<T, 256, 256, 1, 8, 1>(a, nvec, sm_count, blocks_out, st);
-          case 42: return launch_ring_inst<T, 256, 256, 1, 4, 2>(a, nvec, sm_count, blocks_out, st);
-          case 43: return launch_ring_inst<T, 256, 256, 1, 4, 3>(a, nvec, sm_count, blocks_out, st);
-          case 44: return launch_ring_inst<T, 128, 128, 2, 4, 4>(a, nvec, sm_count, blocks_out, st);  // 128-thread CTAs
-          case 45: return launch_ring_inst<T, 128, 128, 2, 4, 3>(a, nvec, sm_count, blocks_out, st);
-          case 46: return launch_ring_inst<T, 256, 128, 2, 4, 2>(a, nvec, sm_count, blocks_out, st);  // 2 row groups x 2 vectors
-          default: return launch_ring_inst<T, 256, 256, 1, 8, 2>(a, nvec, sm_count, blocks_out, st);
+          case 81: return launch_ring_inst<T, 256, 256, 1, 8, 1>(a, bias, nvec, sm_count, blocks_out, st);
+          case 42: return launch_ring_inst<T, 256, 256, 1, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+          case 43: return launch_ring_inst<T, 256, 256, 1, 4, 3>(a, bias, nvec, sm_count, blocks_out, st);
+          case 44: return launch_ring_inst<T, 128, 128, 2, 4, 4>(a, bias, nvec, sm_count, blocks_out, st);  // 128-thread CTAs
+          case 45: return launch_ring_inst<T, 128, 128, 2, 4, 3>(a, bias, nvec, sm_count, blocks_out, st);
+          case 46: return launch_ring_inst<T, 256, 128, 2, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);  // 2 row groups x 2 vectors
+          default: return launch_ring_inst<T, 256, 256, 1, 8, 2>(a, bias, nvec, sm_count, blocks_out, st);
         }
       }
     }
   }
-  if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2>(a, nvec, sm_count, blocks_out, st);
-  return launch_ring_inst<T, 256, 256, 4, 2, 2>(a, nvec, sm_count, blocks_out, st);
+  if (sh.v == 2) return launch_ring_inst<T, 256, 256, 2, 4, 2>(a, bias, nvec, sm_count, blocks_out, st);
+  return launch_ring_inst<T, 256, 256, 4, 2, 2>(a, bias, nvec, sm_count, blocks_out, st);
 }
 
 
@@ -865,17 +903,30 @@ int k1_ring_dual_full_supported(int32_t d, int elem_bytes) {
   return sh.v == 1 && (sh.tpr == 128 || sh.tpr == 256) ? 1 : 0;   // one vector per thread: d <= 1024 (fp32) / 512 (fp64)
 }
 
-cudaError_t k1_ring_launch(const K1Args &a, int elem_bytes, int sm_count, int *blocks_out, cudaStream_t st) {
+cudaError_t k1_ring_launch(const K1Args &a, int bias, int elem_bytes, int sm_count, int *blocks_out, cudaStream_t st) {
   RingShape sh;
   int nvec = 0;
   if (!ring_shape(a.d, elem_bytes, sh, nvec)) return cudaErrorInvalidValue;
   if (a.rows <= 0) { *blocks_out = 0; return cudaSuccess; }
-  if (elem_bytes == 2) return launch_ring_bf16(a, sh, nvec, sm_count, blocks_out, st);
-  if (elem_bytes == 4) return launch_ring_t<float>(a, sh, nvec, sm_count, blocks_out, st);
-  return launch_ring_t<double>(a, sh, nvec, sm_count, blocks_out, st);
+  if (elem_bytes == 2) return launch_ring_bf16(a, bias, sh, nvec, sm_count, blocks_out, st);
+  if (elem_bytes == 4) return launch_ring_t<float>(a, bias, sh, nvec, sm_count, blocks_out, st);
+  return launch_ring_t<double>(a, bias, sh, nvec, sm_count, blocks_out, st);
 }
 
-cudaError_t k1_generic_launch(const K1Args &a, int elem_bytes, int sm_count, int max_blocks, int *blocks_out,
+template <bool BIAS>
+static void k1_generic_launch_t(const K1Args &a, int elem_bytes, unsigned grid, long long ntiles, cudaStream_t st) {
+  if (a.filt) {
+    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, true, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+    else if (elem_bytes == 4) k1_generic_kernel<float, true, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+    else k1_generic_kernel<double, true, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+  } else {
+    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, false, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+    else if (elem_bytes == 4) k1_generic_kernel<float, false, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+    else k1_generic_kernel<double, false, BIAS><<<grid, 256, 0, st>>>(a, ntiles);
+  }
+}
+
+cudaError_t k1_generic_launch(const K1Args &a, int bias, int elem_bytes, int sm_count, int max_blocks, int *blocks_out,
                               cudaStream_t st) {
   if (a.rows <= 0) { *blocks_out = 0; return cudaSuccess; }
   const long long ntiles = (a.rows + 7) / 8;
@@ -884,22 +935,51 @@ cudaError_t k1_generic_launch(const K1Args &a, int elem_bytes, int sm_count, int
   if (grid > ntiles) grid = ntiles;
   if (grid < 1) grid = 1;
   *blocks_out = (int)grid;
-  if (a.filt) {
-    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-    else if (elem_bytes == 4) k1_generic_kernel<float, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-    else k1_generic_kernel<double, true><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+  if (bias) k1_generic_launch_t<true>(a, elem_bytes, (unsigned)grid, ntiles, st);
+  else k1_generic_launch_t<false>(a, elem_bytes, (unsigned)grid, ntiles, st);
+  return cudaGetLastError();
+}
+
+cudaError_t k1_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, const XchgPub *pub, cudaStream_t st,
+                             const double *scale, int32_t scale_d, int32_t blk) {
+  const int grid = (n + 31) / 32;
+  if (scale) {
+    if (pub) k1_reduce_kernel<true, true><<<grid, 256, 0, st>>>(slabs, blocks, n, out, *pub, scale, scale_d, blk);
+    else k1_reduce_kernel<false, true><<<grid, 256, 0, st>>>(slabs, blocks, n, out, XchgPub(), scale, scale_d, blk);
   } else {
-    if (elem_bytes == 2) k1_generic_kernel<__nv_bfloat16, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-    else if (elem_bytes == 4) k1_generic_kernel<float, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
-    else k1_generic_kernel<double, false><<<(unsigned)grid, 256, 0, st>>>(a, ntiles);
+    if (pub) k1_reduce_kernel<true, false><<<grid, 256, 0, st>>>(slabs, blocks, n, out, *pub, nullptr, 0, 1);
+    else k1_reduce_kernel<false, false><<<grid, 256, 0, st>>>(slabs, blocks, n, out, XchgPub(), nullptr, 0, 1);
   }
   return cudaGetLastError();
 }
 
-cudaError_t k1_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, const XchgPub *pub, cudaStream_t st) {
-  const int grid = (n + 31) / 32;
-  if (pub) k1_reduce_kernel<true><<<grid, 256, 0, st>>>(slabs, blocks, n, out, *pub);
-  else k1_reduce_kernel<false><<<grid, 256, 0, st>>>(slabs, blocks, n, out, XchgPub());
+namespace {
+// w_eff = (s o v, b): the point K1 evaluates on the stored features (s o v, then the intercept and the padding copied)
+__global__ void __launch_bounds__(256) transform_point_kernel(double *out, const double *w, double *out2, const double *w2,
+                                                              const double *s, int32_t d, int32_t n) {
+  for (int c = blockIdx.x * 256 + threadIdx.x; c < n; c += gridDim.x * 256) {
+    const double sc = c < d ? s[c] : 1.0;
+    out[c] = c < d ? s[c] * w[c] : w[c];
+    if (out2) out2[c] = c < d ? sc * w2[c] : w2[c];
+  }
+}
+__global__ void __launch_bounds__(256) scale_columns_kernel(double *acc, const double *s, int32_t d) {
+  for (int c = blockIdx.x * 256 + threadIdx.x; c < d; c += gridDim.x * 256) acc[c] *= s[c];
+}
+}  // namespace
+
+cudaError_t transform_point_launch(double *out, const double *w, double *out2, const double *w2, const double *s, int32_t d,
+                                   int32_t n, cudaStream_t st) {
+  int grid = (n + 255) / 256;
+  if (grid > 64) grid = 64;
+  transform_point_kernel<<<grid, 256, 0, st>>>(out, w, out2, w2, s, d, n);
+  return cudaGetLastError();
+}
+
+cudaError_t scale_columns_launch(double *acc, const double *s, int32_t d, cudaStream_t st) {
+  int grid = (d + 255) / 256;
+  if (grid > 64) grid = 64;
+  scale_columns_kernel<<<grid, 256, 0, st>>>(acc, s, d);
   return cudaGetLastError();
 }
 

@@ -178,6 +178,14 @@ __device__ __forceinline__ bool row_kept(unsigned long long seed, unsigned long 
   return row_selected(seed, thresh, grow) && row_in_view(f, grow);
 }
 
+// A load the compiler may not hoist out of a loop: the intercept of a model, read where a margin needs it (an L1 hit) instead
+// of taking a register for the whole row loop of a kernel that has none to spare
+__device__ __forceinline__ double ld_volatile_f64(const double *p) {
+  double v;
+  asm volatile("ld.global.nc.f64 %0, [%1];" : "=d"(v) : "l"(p));
+  return v;
+}
+
 // Transpose-reduce R per-lane partials across a warp: afterwards every lane holds the warp total of
 // row (lane / (32/R)).  R/2 + R/4 + ... + 1 + log2(32/R) 64-bit shuffles instead of 5R.
 template <int R>

@@ -198,7 +198,9 @@ __device__ __forceinline__ unsigned long long pack2(uint32_t lo, uint32_t hi) {
 // operand (hi2, mid2, lo2 for lane j of a quad), so the second X^T r costs no extra MMA instruction; its fp64 gradient
 // lives in shared memory (g2), each entry owned by the one MMA thread that updates it.
 // VIEW: the launch runs on a view (a.filt != nullptr); launches without one take the instantiation without view code.
-template <int RPT, bool F32, int DUAL, bool VIEW>
+// BIAS: the model has an intercept: the scalar warp adds w[d] (w2[d]) to the fp32 / fp64 margin before the loss, and sums the
+// kept rows' multipliers into slot d, so the scalar slots start at d + 1 and a second block at d + 5.
+template <int RPT, bool F32, int DUAL, bool VIEW, bool BIAS>
 __global__ void __launch_bounds__(tc_consumers(RPT) + 256, 1)
 k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap3, const TcArgs a,
              const long long ntiles) {
@@ -266,7 +268,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
    } else if (warp == kCW + 2) {
     // ===================== scalar warp =====================
     // lanes 0-15: the tile's rows at w (loss', loss); DUAL: lanes 16-31 the same rows at w2 (loss only)
-    double lossacc = 0.0, cntacc = 0.0;
+    double lossacc = 0.0, cntacc = 0.0, multacc = 0.0;
     double ynext = 0.0;
     const int srow = lane & 15;
     const bool second = DUAL && lane >= kKR;
@@ -298,6 +300,9 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
           m = (((pp[0] + pp[1]) + (pp[2] + pp[3])) + ((pp[4] + pp[5]) + (pp[6] + pp[7]))) +
               (((pp[8] + pp[9]) + (pp[10] + pp[11])) + ((pp[12] + pp[13]) + (pp[14] + pp[15])));
         }
+        // BIAS: the intercept of this lane's point, loaded where it is added (an L1 hit): a register held across the loop
+        // would make the scalar warp spill under its setmaxnreg budget
+        if (BIAS) m += ld_volatile_f64(second ? a.w2 + a.d : a.w + a.d);
         nonfinite = (lane < kKR || DUAL == 2) && srow < rv && !isfinite(m);
         double mu, loss;
         loss_eval(a.kind, m, ylab, mu, loss);
@@ -306,6 +311,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
         if (srow < rv && (!VIEW || ((a.view_bits[(tile * kKR + srow) >> 5] >> ((tile * kKR + srow) & 31)) & 1u) != 0u) &&
             row_selected(a.sample_seed, a.sample_thresh, a.row_base + tile * kKR + srow)) {
           mult = mu; lossacc += loss; cntacc += 1.0;
+          if (BIAS) multacc += mu;
         }
       }
       named_arrive(3 + bb, kConsumers + 32);                   // partial[bb] may be overwritten
@@ -386,13 +392,19 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
     for (int off = DUAL ? 8 : 16; off >= 1; off >>= 1) {
       lossacc += __shfl_xor_sync(0xffffffffu, lossacc, off);
       cntacc += __shfl_xor_sync(0xffffffffu, cntacc, off);
+      if (BIAS) multacc += __shfl_xor_sync(0xffffffffu, multacc, off);
     }
-    if (lane == 0) { slab[a.d] = lossacc; slab[a.d + 1] = cntacc; if (!DUAL) { slab[a.d + 2] = 0.0; slab[a.d + 3] = 0.0; } }
+    const int DB = a.d + (BIAS ? 1 : 0);
+    if (lane == 0) {
+      if (BIAS) slab[a.d] = multacc;
+      slab[DB] = lossacc; slab[DB + 1] = cntacc; if (!DUAL) { slab[DB + 2] = 0.0; slab[DB + 3] = 0.0; }
+    }
     if (DUAL && lane == kKR) {
-      slab[a.d + 2] = lossacc; slab[a.d + 3] = cntacc;
+      slab[DB + 2] = lossacc; slab[DB + 3] = cntacc;
       if (DUAL == 2) {   // second block: [gradient at w2 | loss sum | count | 0 | 0]
-        double *slab2 = slab + a.d + 4;
-        slab2[a.d] = lossacc; slab2[a.d + 1] = cntacc; slab2[a.d + 2] = 0.0; slab2[a.d + 3] = 0.0;
+        double *slab2 = slab + DB + 4;
+        if (BIAS) slab2[a.d] = multacc;
+        slab2[DB] = lossacc; slab2[DB + 1] = cntacc; slab2[DB + 2] = 0.0; slab2[DB + 3] = 0.0;
       }
     }
    }
@@ -450,7 +462,7 @@ k1_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ C
     for (int p = 0; p < 32; ++p)
       if (p < npairs) {
         slab[128 * p + fo] = gacc[p];
-        if (DUAL == 2) slab[a.d + 4 + 128 * p + fo] = g2[128 * p + fo];
+        if (DUAL == 2) slab[a.d + (BIAS ? 1 : 0) + 4 + 128 * p + fo] = g2[128 * p + fo];
       }
   } else {
     // ===================== consumers: phase 1 in fp64, straight out of the swizzled tile =====================
@@ -689,35 +701,35 @@ cudaError_t set_smem_once(K kern, int bytes) {
   return e;
 }
 
-// the kernel form of a launch (options, second point), with or without view code
-template <bool VIEW>
+// the kernel form of a launch (options, second point), with or without view code and intercept
+template <bool VIEW, bool BIAS>
 cudaError_t tc_launch_forms(const K1Args &a, const CUtensorMap &tmap, const CUtensorMap &tmap3, const TcArgs &t, long long grid,
                             int smem_bytes, long long ntiles, cudaStream_t st) {
   cudaError_t e;
   if (a.tune_rows == 1) {  // option ring_rows=1: row-per-lane consumers (broadcast w reads; measured slower)
-    e = set_smem_once<1 + 8 * VIEW>(k1_tc_kernel<0, false, 0, VIEW>, smem_bytes);
+    e = set_smem_once<1 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<0, false, 0, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<0, false, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<0, false, 0, VIEW, BIAS><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   } else if (a.tune_rows == 4) {  // option ring_rows=4: 256 consumers with four rows each (measured slower)
-    e = set_smem_once<2 + 8 * VIEW>(k1_tc_kernel<4, false, 0, VIEW>, smem_bytes);
+    e = set_smem_once<2 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<4, false, 0, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<4, false, 0, VIEW><<<(unsigned)grid, 512, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<4, false, 0, VIEW, BIAS><<<(unsigned)grid, 512, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   } else if (a.tc_margins_f64) {  // option tc_margins=f64: 512 consumers, two rows per thread, fp64-exact margins
-    e = set_smem_once<3 + 8 * VIEW>(k1_tc_kernel<2, false, 0, VIEW>, smem_bytes);
+    e = set_smem_once<3 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<2, false, 0, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, false, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<2, false, 0, VIEW, BIAS><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   } else if (a.w2 && a.dual_full) {  // the default mapping + loss AND gradient at a second point (speculative sweep)
-    e = set_smem_once<6 + 8 * VIEW>(k1_tc_kernel<2, true, 2, VIEW>, smem_bytes);
+    e = set_smem_once<6 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<2, true, 2, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 2, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<2, true, 2, VIEW, BIAS><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   } else if (a.w2) {  // the default mapping + the loss at a second point (pass fusion)
-    e = set_smem_once<4 + 8 * VIEW>(k1_tc_kernel<2, true, 1, VIEW>, smem_bytes);
+    e = set_smem_once<4 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<2, true, 1, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 1, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<2, true, 1, VIEW, BIAS><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   } else {  // default: the same mapping with fp32 phase-1 arithmetic (fp32 FMAs on packed pairs, no fp64 conversion per element)
-    e = set_smem_once<5 + 8 * VIEW>(k1_tc_kernel<2, true, 0, VIEW>, smem_bytes);
+    e = set_smem_once<5 + 8 * VIEW + 16 * BIAS>(k1_tc_kernel<2, true, 0, VIEW, BIAS>, smem_bytes);
     if (e != cudaSuccess) return e;
-    k1_tc_kernel<2, true, 0, VIEW><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
+    k1_tc_kernel<2, true, 0, VIEW, BIAS><<<(unsigned)grid, 768, smem_bytes, st>>>(tmap, tmap3, t, ntiles);
   }
   return cudaGetLastError();
 }
@@ -730,7 +742,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
 
 int k1_tc_supported(int32_t d, int elem_bytes) { return elem_bytes == 2 && d >= 128 && d <= 4096 && d % 128 == 0; }
 
-cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStream_t st) {
+cudaError_t k1_tc_launch(const K1Args &a, int bias, int sm_count, int *blocks_out, cudaStream_t st) {
   if (!k1_tc_supported(a.d, 2)) return cudaErrorInvalidValue;
   if (a.rows <= 0) { *blocks_out = 0; return cudaSuccess; }
   static EncodeTiledFn encode = nullptr;
@@ -789,8 +801,11 @@ cudaError_t k1_tc_launch(const K1Args &a, int sm_count, int *blocks_out, cudaStr
   if (grid > ntiles) grid = ntiles;
   *blocks_out = (int)grid;
   const int smem_bytes = (int)L.total + 1024;
-  return a.filt ? tc_launch_forms<true>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st)
-                : tc_launch_forms<false>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st);
+  if (bias)
+    return a.filt ? tc_launch_forms<true, true>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st)
+                  : tc_launch_forms<false, true>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st);
+  return a.filt ? tc_launch_forms<true, false>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st)
+                : tc_launch_forms<false, false>(a, tmap, tmap3, t, grid, smem_bytes, ntiles, st);
 }
 
 }  // namespace agd

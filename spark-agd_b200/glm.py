@@ -179,10 +179,12 @@ class GeneralizedLinearAlgorithm:
         # both switches rewrite every row (appendBias / StandardScaler); the resident shard is used as it is
         if self.addIntercept:
             raise ValueError("run(DeviceDataset) cannot add an intercept: it needs a copy of the resident shard with a "
-                             "column of ones appended; train from host rows (run(sc, labels, X)) instead")
+                             "column of ones appended; train from host rows (run(sc, labels, X)) instead, or train on "
+                             "the view MLUtils.appendBias(data), whose last weight is the intercept")
         if self.useFeatureScaling:
             raise ValueError("run(DeviceDataset) cannot scale features: it needs a rescaled copy of the resident shard; "
-                             "train from host rows (run(sc, labels, X)) instead")
+                             "train from host rows (run(sc, labels, X)) instead, or train on the view "
+                             "StandardScaler().fit(data).transform(data)")
         d = data.d
         w0 = np.zeros(d) if initialWeights is None else np.asarray(initialWeights, dtype=np.float64)
         if w0.ndim != 1 or w0.shape[0] != d:

@@ -222,7 +222,14 @@ class DeviceDataset:
     rows by a fixed predicate on each row's own random draw, without copying a row.  Every compute call on a view (smooth*,
     evaluate, margins, training) sets the view's filter on the handle for that call only; close() on a view frees nothing.
     The accessors that address PHYSICAL rows -- local_rows, get_rows, get_labels, get_csr_rows, margins_rows -- return the
-    parent's rows on a view as well (the view's own rows of them: row_mask; its row count: count())."""
+    parent's rows on a view as well (the view's own rows of them: row_mask; its row count: count()).
+
+    StandardScalerModel.transform and MLUtils.appendBias return views too: features scaled by s and / or a constant 1.0
+    appended, computed on the stored rows without rewriting them (agd_set_feature_transform).  `d` reports the transformed
+    width; the physical-row accessors still return the stored features.  Transforms and row views compose in either order."""
+
+    _scale = None      # a transformed view: the factor s of every stored feature (None: unscaled) ...
+    _bias = False      # ... and whether a constant 1.0 is appended as the last feature
 
     def __init__(self, ctx: Context):
         self.ctx = ctx
@@ -233,12 +240,13 @@ class DeviceDataset:
         self._preds = ()       # a view: its predicates (seed, lo, hi, complement)
 
     def _view(self, pred) -> "DeviceDataset":
-        preds = self._preds + (pred,)
+        preds = self._preds + ((pred,) if pred is not None else ())
         if len(preds) > MAX_VIEW_PREDICATES:
             raise ValueError(f"a view nests at most {MAX_VIEW_PREDICATES} predicates (randomSplit / sample / kFold levels)")
-        seed, lo, hi, comp = pred
-        if not (0.0 <= lo <= hi <= 1.0):
-            raise ValueError(f"bounds must satisfy 0 <= lo <= hi <= 1, got [{lo}, {hi})")
+        if pred is not None:
+            seed, lo, hi, comp = pred
+            if not (0.0 <= lo <= hi <= 1.0):
+                raise ValueError(f"bounds must satisfy 0 <= lo <= hi <= 1, got [{lo}, {hi})")
         v = object.__new__(DeviceDataset)
         v.ctx = self.ctx
         v._base = self._base if self._base is not None else self
@@ -246,28 +254,62 @@ class DeviceDataset:
         v.total_rows = v._base.total_rows
         v._xchg_d = 0
         v._preds = preds
+        v._scale, v._bias = self._scale, self._bias
         return v
+
+    def _transformed(self, scale=None, bias: bool = False) -> "DeviceDataset":
+        """A view with the stored features multiplied by `scale` and / or a constant 1.0 appended (MLlib's order: scale,
+        then appendBias).  It keeps this dataset's rows; a row view of it keeps the transform."""
+        if self._bias:
+            raise ValueError("this view already ends in the appended bias column: appendBias comes last, after any scaling")
+        if scale is not None and self._scale is not None:
+            raise ValueError("this view is already scaled; fit and apply one StandardScalerModel")
+        v = self._view(None)
+        if scale is not None:
+            scale = np.array(scale, dtype=np.float64, copy=True)
+            if scale.ndim != 1 or scale.shape[0] != self._phys_d:
+                raise ValueError(f"scale has size {scale.shape}, data has {self._phys_d} features")
+            if not np.all(np.isfinite(scale)):
+                raise ValueError("scale factors must be finite")
+            scale.setflags(write=False)
+            v._scale = scale
+        v._bias = self._bias or bool(bias)
+        return v
+
+    def _physical_model(self, w, intercept: float):
+        """A model of this view's features as a model of the stored ones (what agd_margins / agd_evaluate score)."""
+        return physical_model(w, intercept, self._scale, self._bias)
 
     @property
     def is_view(self) -> bool:
         return self._base is not None
 
     def _filtered(self):
-        """Context manager: the view's filter is on the handle for the duration of one call, and cleared afterwards, also on
-        error (the parent and sibling views never see it).  A dataset that is not a view leaves the handle alone."""
+        """Context manager: the view's filter and feature transform are on the handle for the duration of one call, and
+        cleared afterwards, also on error (the parent and sibling views never see them).  A dataset that is not a view leaves
+        the handle alone."""
         ds = self
+        transformed = ds._scale is not None or ds._bias
 
         class _F:
             def __enter__(self_):
-                if ds._preds:
-                    n = len(ds._preds)
-                    seeds = np.array([p[0] for p in ds._preds], dtype=np.uint64)
-                    lo = np.array([p[1] for p in ds._preds], dtype=np.float64)
-                    hi = np.array([p[2] for p in ds._preds], dtype=np.float64)
-                    comp = np.array([1 if p[3] else 0 for p in ds._preds], dtype=np.int32)
-                    N.check(N.lib().agd_set_row_filter(ds.h, n, _ptr(seeds), _ptr(lo), _ptr(hi), _ptr(comp)), ds.h)
+                try:
+                    if ds._preds:
+                        n = len(ds._preds)
+                        seeds = np.array([p[0] for p in ds._preds], dtype=np.uint64)
+                        lo = np.array([p[1] for p in ds._preds], dtype=np.float64)
+                        hi = np.array([p[2] for p in ds._preds], dtype=np.float64)
+                        comp = np.array([1 if p[3] else 0 for p in ds._preds], dtype=np.int32)
+                        N.check(N.lib().agd_set_row_filter(ds.h, n, _ptr(seeds), _ptr(lo), _ptr(hi), _ptr(comp)), ds.h)
+                    if transformed:
+                        N.check(N.lib().agd_set_feature_transform(ds.h, _ptr(ds._scale), int(ds._bias)), ds.h)
+                except BaseException:
+                    self_.__exit__()
+                    raise
 
             def __exit__(self_, *exc):
+                if transformed:
+                    N.check(N.lib().agd_set_feature_transform(ds.h, None, 0), ds.h)
                 if ds._preds:
                     N.check(N.lib().agd_set_row_filter(ds.h, 0, None, None, None, None), ds.h)
                 return False
@@ -373,8 +415,14 @@ class DeviceDataset:
         self.total_rows += n
 
     @property
-    def d(self) -> int:
+    def _phys_d(self) -> int:
+        """Features as stored (what the physical-row accessors return)."""
         return int(N.lib().agd_dim(self.h))
+
+    @property
+    def d(self) -> int:
+        """Features of this dataset: the stored ones, plus the appended bias column on a view that has one."""
+        return self._phys_d + (1 if self._bias else 0)
 
     def local_rows(self, dev: int = 0) -> int:
         """Physical rows of local device `dev`'s shard (on a view too: the parent's)."""
@@ -382,8 +430,9 @@ class DeviceDataset:
 
     def get_rows(self, dev: int, row0: int, rows: int, dtype=np.float32):
         """Physical rows as stored (dtype must match the storage: float32, float64, or uint16 for raw bf16); on a view, the
-        parent's rows [row0, row0 + rows) -- select the view's with row_mask(dev, row0, rows)."""
-        X = np.empty((rows, self.d), dtype=dtype)
+        parent's rows [row0, row0 + rows) -- select the view's with row_mask(dev, row0, rows).  A transformed view returns
+        the stored features too (neither scaled nor with the bias column)."""
+        X = np.empty((rows, self._phys_d), dtype=dtype)
         y = np.empty(rows, dtype=np.float64)
         N.check(N.lib().agd_get_rows(self.h, dev, row0, rows, _ptr(X), _ptr(y)), self.h)
         return X, y
@@ -463,8 +512,8 @@ class DeviceDataset:
 
     def margins_rows(self, dev: int, row0: int, rows: int, w, intercept: float = 0.0) -> np.ndarray:
         """x_i . w + intercept (fp64) of physical rows [row0, row0 + rows) of local device `dev`'s shard (not collective; on a
-        view too, see margins for the view's rows)."""
-        w = self._weights(w)
+        view too, see margins for the view's rows).  On a transformed view x_i is the transformed row."""
+        w, intercept = self._physical_model(self._weights(w), intercept)
         out = np.empty(max(int(rows), 0), dtype=np.float64)
         N.check(N.lib().agd_margins(self.h, dev, _ptr(w), float(intercept), int(row0), int(rows), _ptr(out)), self.h)
         return out
@@ -481,7 +530,7 @@ class DeviceDataset:
     def evaluate(self, gradient: Gradient, w, intercept: float = 0.0, threshold: float = 0.5) -> "Evaluation":
         """Loss, confusion counts and error moments of the model (w, intercept) over every shard of the world, from one
         read of X (collective: every rank calls it; every rank gets the same bits)."""
-        w = self._weights(w)
+        w, intercept = self._physical_model(self._weights(w), intercept)
         sums = np.empty(N.EVAL_N, dtype=np.float64)
         self._ensure_exchange()
         with self._filtered():
@@ -548,6 +597,16 @@ class MLUtils:
         return ds
 
     @staticmethod
+    def appendBias(x):
+        """MLUtils.appendBias: a constant 1.0 as the last feature.  On a host matrix (or vector) a new array; on a DeviceDataset
+        a view with d + 1 features that rewrites no row (the intercept is the last weight of a model trained on it)."""
+        if isinstance(x, DeviceDataset):
+            return x._transformed(bias=True)
+        from .glm import append_bias
+        x = np.asarray(x)
+        return append_bias(x) if x.ndim == 2 else append_bias(x[None, :])[0]
+
+    @staticmethod
     def kFold(data: "DeviceDataset", numFolds: int, seed: int = DEFAULT_SPLIT_SEED) -> list:
         """MLUtils.kFold(rdd, numFolds, seed): numFolds (training, validation) pairs of views; validation i keeps the rows
         whose draw lies in [i / k, (i + 1) / k), training i is its complement."""
@@ -559,6 +618,16 @@ class MLUtils:
             lo, hi = i / k, (i + 1) / k
             out.append((data._view((int(seed), lo, hi, True)), data._view((int(seed), lo, hi, False))))
         return out
+
+
+def physical_model(w, intercept: float, scale=None, bias: bool = False):
+    """(w, intercept) of a model on appendBias(s o x) as a model on the stored x: (s o v, intercept + b), where v are the
+    feature weights and b the bias column's weight (the last of w when bias)."""
+    w = np.asarray(w, dtype=np.float64)
+    v, b = (w[:-1], float(w[-1])) if bias else (w, 0.0)
+    if scale is not None:
+        v = v * np.asarray(scale, dtype=np.float64)
+    return np.ascontiguousarray(v), float(intercept) + b
 
 
 def _ratio(a: float, b: float) -> float:

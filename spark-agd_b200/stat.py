@@ -83,6 +83,22 @@ class MultivariateStatisticalSummary:
     def normL2(self) -> np.ndarray:
         return np.sqrt(self.sum_sq)
 
+    def transformed(self, scale=None, bias: bool = False) -> "MultivariateStatisticalSummary":
+        """The summary of appendBias(s o x) from that of x, in O(d): sums scale by s, squares by s^2 (so mean, max, min, normL1
+        and normL2 scale by |s| -- max and min swap where s < 0 -- and the variance by s^2); a column with s = 0 has no
+        nonzeros.  The bias column: count rows of 1.0 (mean 1, variance 0, max = min = 1, normL1 = n, normL2 = sqrt(n))."""
+        cols = [self.sum, self.sum_sq, self.sum_abs, self.nnz, self.dev, self.dev2, self.col_max, self.col_min]
+        if scale is not None:
+            s = np.asarray(scale, dtype=np.float64)
+            neg = s < 0
+            hi, lo = self.col_max * s, self.col_min * s
+            cols = [self.sum * s, self.sum_sq * (s * s), self.sum_abs * np.abs(s), np.where(s != 0, self.nnz, 0.0),
+                    self.dev * s, self.dev2 * (s * s), np.where(neg, lo, hi), np.where(neg, hi, lo)]
+        if bias:
+            n = self.n
+            cols = [np.append(c, v) for c, v in zip(cols, [n, n, n, n, 0.0, 0.0, 1.0, 1.0])]
+        return MultivariateStatisticalSummary.from_sums(self.n, np.stack(cols))
+
 
 class Statistics:
     """org.apache.spark.mllib.stat.Statistics [mllib-1.3.0] (column summaries)."""
@@ -90,11 +106,15 @@ class Statistics:
     @staticmethod
     def colStats(data: DeviceDataset) -> MultivariateStatisticalSummary:
         """Column statistics of a DeviceDataset or view over every shard of the world (collective: every rank calls it and
-        every rank gets the same bits).  A view's filter is set for this call only."""
-        d = data.d
+        every rank gets the same bits).  A view's filter is set for this call only.  On a transformed view the statistics
+        are those of the transformed features, derived from the stored features' (MultivariateStatisticalSummary.transformed)."""
+        d = data._phys_d
         sums = np.empty((N.COLSTAT_N, d), dtype=np.float64)
         count = C.c_double()
         data._ensure_exchange()
         with data._filtered():
             N.check(N.lib().agd_col_stats(data.h, C.byref(count), _ptr(sums)), data.h)
-        return MultivariateStatisticalSummary.from_sums(count.value, sums)
+        summary = MultivariateStatisticalSummary.from_sums(count.value, sums)
+        if data._scale is not None or data._bias:
+            summary = summary.transformed(data._scale, data._bias)
+        return summary
