@@ -215,6 +215,23 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
 enum { AGD_COLSTAT_SUM = 0, AGD_COLSTAT_SUM_SQ, AGD_COLSTAT_SUM_ABS, AGD_COLSTAT_NNZ,
        AGD_COLSTAT_DEV, AGD_COLSTAT_DEV2, AGD_COLSTAT_MAX, AGD_COLSTAT_MIN, AGD_COLSTAT_N };
 int agd_col_stats(agd_handle *h, double *count, double *out);
+/* Ranking metrics over ALL shards of the world (BinaryClassificationMetrics of mllib 1.3.0; collective, like agd_evaluate).
+ * Rows: every row of the current view (agd_set_row_filter applies; agd_set_feature_transform does not: score a transformed
+ * model with weights s o v and intercept b, as for agd_evaluate); a row outside the view leaves no trace.  A row is positive
+ * iff label > 0.5.  Its score is the fp64 margin m = x . w + intercept with exactly the bits agd_margins returns, -0 taken as
+ * +0; a row whose margin is NaN is only counted (AGD_BIN_NAN) and left out of the curve.
+ * The curve has one point per distinct score, in descending order, with the cumulative counts TP_k / FP_k of the rows scoring
+ * at least that much.  With P positives and N negatives, ROC = (0, 0), (FP_k / N, TP_k / P) ..., (1, 1) and PR = (0, 1),
+ * (TP_k / P, TP_k / (TP_k + FP_k)) ...; the areas are trapezoid sums over those points, fp64 in a fixed order (the bits depend
+ * on the curve only: identical on every rank, every repeated call, every partitioning of the same rows, dense or CSR).
+ * AUROC is NaN when P = 0 or N = 0, AUPR when P = 0.  Counts are exact.
+ * w: agd_dim(h) doubles; out: AGD_BIN_N doubles; *n_points = points of the curve.  The curve (margin_out descending, tp_out,
+ * fp_out cumulative) is written only when capacity >= *n_points; capacity 0 asks for the areas only.  Scratch memory (about
+ * 18 bytes per local row, and 48 bytes per distinct score of the world on the first local device) stays on the handle until
+ * agd_clear / agd_destroy. */
+enum { AGD_BIN_POS = 0, AGD_BIN_NEG, AGD_BIN_NAN, AGD_BIN_AUROC, AGD_BIN_AUPR, AGD_BIN_N };
+int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t capacity, double *margin_out, int64_t *tp_out,
+                     int64_t *fp_out, int64_t *n_points, double *out);
 
 /* ---- views of the resident shards (RDD.randomSplit / sample / MLUtils.kFold without copying a row) ----
  * Every row has a 64-bit draw u = Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, 7), words 0 and 1, where grow
@@ -223,7 +240,7 @@ int agd_col_stats(agd_handle *h, double *count, double *out);
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask), agd_evaluate and agd_col_stats, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate, agd_col_stats and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */

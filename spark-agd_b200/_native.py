@@ -21,6 +21,8 @@ XCHG_HANDLE_BYTES = 192
 # agd_evaluate: indices of the sums it returns (AGD_EVAL_*), EVAL_N of them
 (EVAL_COUNT, EVAL_LOSS, EVAL_TP, EVAL_FP, EVAL_TN, EVAL_FN, EVAL_SUM_ERR, EVAL_SUM_ERR2, EVAL_SUM_ABS_ERR, EVAL_SUM_Y,
  EVAL_SUM_Y2, EVAL_N) = range(12)
+# agd_binary_curve: the summary it returns (AGD_BIN_*), BIN_N doubles
+BIN_POS, BIN_NEG, BIN_NAN, BIN_AUROC, BIN_AUPR, BIN_N = range(6)
 # agd_col_stats: rows of the statistic-major block it returns (AGD_COLSTAT_*), COLSTAT_N of them
 (COLSTAT_SUM, COLSTAT_SUM_SQ, COLSTAT_SUM_ABS, COLSTAT_NNZ, COLSTAT_DEV, COLSTAT_DEV2, COLSTAT_MAX, COLSTAT_MIN,
  COLSTAT_N) = range(9)
@@ -115,6 +117,8 @@ _SIGNATURES = {
     "agd_margins": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_evaluate": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
     "agd_col_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
+    "agd_binary_curve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.POINTER(C.c_int64), C.c_void_p]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "agd_row_filter_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_set_feature_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

@@ -10,6 +10,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -77,6 +78,21 @@ struct Shard {
   int64_t nnz = 0, nnz_cap = 0;
 };
 
+// agd_binary_curve's scratch buffers on a device
+enum BinBuf {
+  kBinKeys0, kBinKeys1,   // keys of a sort (ping-pong): the view's rows, then on device 0 the world's concatenated lists
+  kBinVals0, kBinVals1,   // their values: classes (1 byte), then indices (4 bytes)
+  kBinMisc,               // [8 x 256 digit counts | counters (2 u32) | runs (i64) | areas (2) | own {len, nan} (2) | world's {len, nan} | offsets]
+  kBinTiles,              // per-tile digit counts / sums of the scans / area partials
+  kBinList,               // this device's curve: BinRec per distinct key
+  kBinUnion,              // the world's lists, rank r's at r * (longest list)
+  kBinCounts,             // each concatenated record's own counts: pos [T] | neg [T]
+  kBinCurve,              // the world's curve
+  kBinBufs
+};
+constexpr size_t kBinMiscCounters = 8 * 256 * sizeof(unsigned), kBinMiscRuns = kBinMiscCounters + 8,
+                 kBinMiscAreas = kBinMiscRuns + 8, kBinMiscOwn = kBinMiscAreas + 16, kBinMiscAll = kBinMiscOwn + 16;
+
 struct Dev {
   int ordinal = -1;
   int sm_count = 0;
@@ -91,6 +107,8 @@ struct Dev {
   double *eval = nullptr;          // AGD_EVAL_N sums of agd_evaluate (this shard's, then the world's)
   double *cs = nullptr;            // agd_col_stats: pass-1 sums, maxima, pass-2 sums, CSR max keys (see colstats_layout)
   size_t cs_doubles = 0;
+  void *bin[kBinBufs] = {};        // agd_binary_curve scratch (see BinBuf), grown on demand, freed by agd_clear / agd_destroy
+  size_t bin_bytes[kBinBufs] = {};
   double *partials = nullptr;
   unsigned int *ticket = nullptr;
   double *scalars_dev = nullptr;   // device alias of scalars_host: K3 writes its scalars straight to the host
@@ -336,6 +354,26 @@ int ensure_stage(agd_handle *h, Dev &D, size_t bytes) {
   return 0;
 }
 
+int ensure_bin(agd_handle *h, Dev &D, int which, size_t bytes) {
+  if (D.bin_bytes[which] >= bytes) return 0;
+  if (D.bin[which]) cudaFree(D.bin[which]);
+  D.bin[which] = nullptr;
+  D.bin_bytes[which] = 0;
+  if (cudaMalloc(&D.bin[which], bytes) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(h, "agd_binary_curve: cannot allocate %zu bytes of scratch on device %d", bytes, D.ordinal);
+  }
+  D.bin_bytes[which] = bytes;
+  return 0;
+}
+void free_bin(Dev &D) {
+  for (int i = 0; i < kBinBufs; ++i) {
+    if (D.bin[i]) cudaFree(D.bin[i]);
+    D.bin[i] = nullptr;
+    D.bin_bytes[i] = 0;
+  }
+}
+
 // The current filter as a bitmap of D's rows, drawn by the kernels' own row_in_view() (one launch, one Philox per row and
 // predicate): rebuilt when the filter, the shard's row count or its row numbering changed since the last build, so a run of
 // many sweeps on one view draws its rows once.  One bit per row (rows / 8 bytes next to the shard).
@@ -429,7 +467,7 @@ int ensure_nccl(agd_handle *h) {
 int xchg_alloc(agd_handle *h, std::vector<XHandles> &mine) {
   const int W = h->world, nd = (int)h->devs.size();
   const int S = xchg_slot_stride(h->d);      // slot stride: room for a two-gradient sweep or an evaluation
-  const size_t total = xchg_total_doubles(S, W), nflags = 6 * (size_t)W;   // one-shot + reduce-scatter areas (agd_common.cuh)
+  const size_t total = xchg_alloc_doubles(S, W), nflags = 6 * (size_t)W;   // one-shot, reduce-scatter and bulk areas (agd_common.cuh)
   mine.assign((size_t)nd, XHandles());
   for (int i = 0; i < nd; ++i) {
     Dev &D = h->devs[i];
@@ -956,6 +994,7 @@ int agd_destroy(agd_handle *h) {
     if (D.stage_dev) cudaFree(D.stage_dev);
     if (D.filt_dev) cudaFree(D.filt_dev);
     if (D.view_bits) cudaFree(D.view_bits);
+    free_bin(D);
     for (cudaEvent_t e : D.ev) cudaEventDestroy(e);
     for (cudaEvent_t e : D.ev_ar) cudaEventDestroy(e);
     if (&D == &h->devs[0] && h->ev_begin) { cudaEventDestroy(h->ev_begin); cudaEventDestroy(h->ev_end); }
@@ -1271,6 +1310,7 @@ int agd_clear(agd_handle *h) {
     CK(cudaSetDevice(D.ordinal));
     CK(cudaStreamSynchronize(D.st));
     if (free_shard(h, D)) return 1;
+    free_bin(D);
   }
   h->d = 0;
   h->d_user = 0;
@@ -1674,6 +1714,223 @@ int agd_col_stats(agd_handle *h, double *count, double *out) {
     }
     const double v[AGD_COLSTAT_N] = {sum, r[d + c], r[2 * (size_t)d + c], r[3 * (size_t)d + c], dev, dev2, mx, -nmn};
     for (int k = 0; k < AGD_COLSTAT_N; ++k) out[(size_t)k * du + c] = v[k];
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------- ranking metrics (rank.cu)
+// One shard: the key form of the scoring sweep (rows of the view, non-NaN margins), the radix sort and the run-length reduce
+// into this device's curve (D.bin[kBinList], *len records); *nan = rows of the view whose margin is NaN.
+static int bin_local(agd_handle *h, Dev &D, double intercept, int64_t *len, int64_t *nan) {
+  const int64_t rows = D.sh.rows;
+  if (rows >= (int64_t)1 << 31) return fail(h, "agd_binary_curve: %lld rows on device %d (at most 2^31 - 1)", (long long)rows, D.ordinal);
+  const size_t r1 = rows > 0 ? (size_t)rows : 1;
+  if (ensure_bin(h, D, kBinMisc, kBinMiscAll + 16 * (size_t)h->world + 8 * ((size_t)h->world + 1)) ||
+      ensure_bin(h, D, kBinKeys0, 8 * r1) || ensure_bin(h, D, kBinKeys1, 8 * r1) || ensure_bin(h, D, kBinVals0, r1) ||
+      ensure_bin(h, D, kBinVals1, r1))
+    return 1;
+  char *misc = (char *)D.bin[kBinMisc];
+  unsigned *counters = (unsigned *)(misc + kBinMiscCounters);
+  CK(cudaMemsetAsync(counters, 0, 2 * sizeof(unsigned), D.st));
+  ScoreArgs a = score_args(h, D, intercept);
+  a.rows = rows; a.row_base = D.row_base; a.filt = h->filt_of(D);
+  a.keys = (unsigned long long *)D.bin[kBinKeys0]; a.classes = (uint8_t *)D.bin[kBinVals0]; a.counters = counters;
+  CK(score_keys_launch(a, D.sh.elem_bytes, D.sm_count));
+  unsigned cnt[2];
+  CK(cudaMemcpyAsync(cnt, counters, sizeof cnt, cudaMemcpyDeviceToHost, D.st));
+  CK(cudaStreamSynchronize(D.st));
+  const long long n = cnt[0];
+  *nan = cnt[1];
+  if (ensure_bin(h, D, kBinTiles, std::max(bin_sort_tile_words(n) * sizeof(unsigned), bin_runs_tile_words(n) * sizeof(long long))) ||
+      ensure_bin(h, D, kBinList, (n > 0 ? (size_t)n : 1) * sizeof(BinRec)))
+    return 1;
+  unsigned long long *keys[2] = {(unsigned long long *)D.bin[kBinKeys0], (unsigned long long *)D.bin[kBinKeys1]};
+  void *vals[2] = {D.bin[kBinVals0], D.bin[kBinVals1]};
+  int which = 0, passes = 0;
+  CK(bin_sort_pairs(keys, vals, 1, n, (unsigned *)misc, (unsigned *)D.bin[kBinTiles], &which, &passes, D.st));
+  long long *runs = (long long *)(misc + kBinMiscRuns);
+  CK(bin_runs_launch(keys[which], vals[which], 1, nullptr, nullptr, n, (long long *)D.bin[kBinTiles], (BinRec *)D.bin[kBinList],
+                     runs, D.st));
+  long long k = 0;
+  CK(cudaMemcpyAsync(&k, runs, sizeof k, cudaMemcpyDeviceToHost, D.st));
+  CK(cudaStreamSynchronize(D.st));
+  *len = k;
+  return 0;
+}
+
+// Every rank's list -> the world's curve on device 0 (*curve, *K records), identical on every rank: the lengths travel first
+// (a copy epoch of the exchange, or an NCCL all-gather), then the lists (rank r's at r * Lmax in kBinUnion: copy epochs through
+// the exchange's bulk area, or one all-gather); device 0 concatenates them in rank order, sorts and reduces again.
+static int bin_world(agd_handle *h, const std::vector<int64_t> &len, const std::vector<int64_t> &nan, BinRec **curve,
+                     int64_t *K, int64_t *nan_total) {
+  const int W = h->world, nd = (int)h->devs.size();
+  const bool p2p = h->x_p2p;
+  const int S = xchg_slot_stride(h->d);
+  NcclApi &N = nccl_api();
+  if (!p2p && (!h->comm_ready || !h->devs[0].comm))
+    return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", W);
+  // 1. {list length, NaN count} of every rank
+  const unsigned long long e0 = p2p ? ++h->x_epoch : 0ull;
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    double *own = (double *)((char *)D.bin[kBinMisc] + kBinMiscOwn);
+    const double v[2] = {(double)len[i], (double)nan[i]};
+    CK(cudaMemcpyAsync(own, v, sizeof v, cudaMemcpyHostToDevice, D.st));
+    CK(cudaStreamSynchronize(D.st));   // v is on this stack frame
+    if (p2p) {
+      XchgPub pub;
+      pub.peers = D.xpeers; pub.world = W; pub.my_rank = h->first_rank + i; pub.buf = (int)(e0 & 1ull);
+      pub.n = 2; pub.slot_stride = S; pub.epoch = e0; pub.ticket = D.xticket;
+      CK(xchg_publish_launch(own, pub, D.st));
+    }
+  }
+  if (p2p) {
+    for (Dev &D : h->devs) {
+      CK(cudaSetDevice(D.ordinal));
+      CK(xchg_gather_copy_launch(D.xbuf, D.xflags, W, (int)(e0 & 1ull), 2, S, e0, (double *)((char *)D.bin[kBinMisc] + kBinMiscAll), 2, D.st));
+    }
+  } else {
+    CKN(N.GroupStart());
+    for (Dev &D : h->devs) {
+      char *misc = (char *)D.bin[kBinMisc];
+      CKN(N.AllGather(misc + kBinMiscOwn, misc + kBinMiscAll, 2, ncclDouble, D.comm, D.st));
+    }
+    CKN(N.GroupEnd());
+  }
+  std::vector<double> all((size_t)2 * W);
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  CK(cudaMemcpyAsync(all.data(), (char *)D0.bin[kBinMisc] + kBinMiscAll, all.size() * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  std::vector<long long> off((size_t)W + 1, 0);
+  long long lmax = 0, nans = 0;
+  for (int r = 0; r < W; ++r) {
+    const long long l = (long long)all[2 * (size_t)r];
+    off[(size_t)r + 1] = off[(size_t)r] + l;
+    lmax = std::max(lmax, l);
+    nans += (long long)all[2 * (size_t)r + 1];
+  }
+  const long long T = off[(size_t)W];
+  *nan_total = nans;
+  *K = 0;
+  if (T == 0) return 0;
+  if (T >= (long long)1 << 31) return fail(h, "agd_binary_curve: %lld distinct scores over the world (at most 2^31 - 1)", T);
+  // 2. the lists
+  const size_t ld = 3 * (size_t)lmax;   // doubles of one rank's block
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    if (ensure_bin(h, D, kBinUnion, (size_t)W * ld * sizeof(double))) return 1;
+    double *mine = (double *)D.bin[kBinUnion] + (size_t)(h->first_rank + i) * ld;
+    if (len[i] > 0) CK(cudaMemcpyAsync(mine, D.bin[kBinList], (size_t)len[i] * sizeof(BinRec), cudaMemcpyDeviceToDevice, D.st));
+  }
+  if (p2p) {
+    const size_t off_bulk = xchg_off_bulk(S, W);
+    for (size_t c0 = 0; c0 < ld; c0 += kXchgBulk) {
+      const int m = (int)std::min((size_t)kXchgBulk, ld - c0);
+      const unsigned long long e = ++h->x_epoch;
+      for (int i = 0; i < nd; ++i) {
+        Dev &D = h->devs[i];
+        CK(cudaSetDevice(D.ordinal));
+        XchgPub pub;
+        pub.peers = D.xpeers;
+        for (int r = 0; r < W; ++r) pub.peers.slot[r] += off_bulk;
+        pub.world = W; pub.my_rank = h->first_rank + i; pub.buf = (int)(e & 1ull);
+        pub.n = m; pub.slot_stride = kXchgBulk; pub.epoch = e; pub.ticket = D.xticket;
+        CK(xchg_publish_launch((double *)D.bin[kBinUnion] + (size_t)pub.my_rank * ld + c0, pub, D.st));
+      }
+      for (Dev &D : h->devs) {
+        CK(cudaSetDevice(D.ordinal));
+        CK(xchg_gather_copy_launch(D.xbuf + off_bulk, D.xflags, W, (int)(e & 1ull), m, kXchgBulk, e, (double *)D.bin[kBinUnion] + c0,
+                                   ld, D.st));
+      }
+    }
+  } else {
+    CKN(N.GroupStart());
+    for (int i = 0; i < nd; ++i) {
+      Dev &D = h->devs[i];
+      double *u = (double *)D.bin[kBinUnion];
+      CKN(N.AllGather(u + (size_t)(h->first_rank + i) * ld, u, ld, ncclDouble, D.comm, D.st));   // moves bytes: no arithmetic
+    }
+    CKN(N.GroupEnd());
+  }
+  // 3. device 0: the concatenation in rank order, sorted and reduced
+  CK(cudaSetDevice(D0.ordinal));
+  const size_t t1 = (size_t)T;
+  if (ensure_bin(h, D0, kBinKeys0, 8 * t1) || ensure_bin(h, D0, kBinKeys1, 8 * t1) || ensure_bin(h, D0, kBinVals0, 4 * t1) ||
+      ensure_bin(h, D0, kBinVals1, 4 * t1) || ensure_bin(h, D0, kBinCounts, 16 * t1) ||
+      ensure_bin(h, D0, kBinCurve, t1 * sizeof(BinRec)) ||
+      ensure_bin(h, D0, kBinTiles, std::max(bin_sort_tile_words(T) * sizeof(unsigned), bin_runs_tile_words(T) * sizeof(long long))))
+    return 1;
+  char *misc = (char *)D0.bin[kBinMisc];
+  long long *off_dev = (long long *)(misc + kBinMiscAll + 16 * (size_t)W);
+  CK(cudaMemcpyAsync(off_dev, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice, D0.st));
+  long long *upos = (long long *)D0.bin[kBinCounts], *uneg = upos + T;
+  unsigned long long *keys[2] = {(unsigned long long *)D0.bin[kBinKeys0], (unsigned long long *)D0.bin[kBinKeys1]};
+  void *vals[2] = {D0.bin[kBinVals0], D0.bin[kBinVals1]};
+  CK(bin_union_prep_launch((const BinRec *)D0.bin[kBinUnion], lmax, off_dev, W, T, keys[0], (uint32_t *)vals[0], upos, uneg, D0.st));
+  int which = 0, passes = 0;
+  CK(bin_sort_pairs(keys, vals, 4, T, (unsigned *)misc, (unsigned *)D0.bin[kBinTiles], &which, &passes, D0.st));   // synchronises
+  long long *runs = (long long *)(misc + kBinMiscRuns);
+  CK(bin_runs_launch(keys[which], vals[which], 4, upos, uneg, T, (long long *)D0.bin[kBinTiles], (BinRec *)D0.bin[kBinCurve], runs,
+                     D0.st));
+  long long k = 0;
+  CK(cudaMemcpyAsync(&k, runs, sizeof k, cudaMemcpyDeviceToHost, D0.st));
+  CK(cudaStreamSynchronize(D0.st));
+  *curve = (BinRec *)D0.bin[kBinCurve];
+  *K = k;
+  return 0;
+}
+
+// Collective: the local curves, their union over the world, the areas on device 0; the curve is copied out only on request.
+int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t capacity, double *margin_out, int64_t *tp_out,
+                     int64_t *fp_out, int64_t *n_points, double *out) {
+  if (check_ready(h)) return 1;
+  if (!w || !n_points || !out) return fail(h, "NULL argument");
+  if (capacity < 0) return fail(h, "capacity must be >= 0 (got %lld)", (long long)capacity);
+  if (capacity > 0 && (!margin_out || !tp_out || !fp_out)) return fail(h, "NULL argument");
+  h->xg_pending = false;
+  const int nd = (int)h->devs.size();
+  std::vector<int64_t> len((size_t)nd), nan((size_t)nd);
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    if (stage_weights(h, D, w)) return 1;
+    if (bin_local(h, D, intercept, &len[(size_t)i], &nan[(size_t)i])) return 1;
+  }
+  Dev &D0 = h->devs[0];
+  BinRec *curve = (BinRec *)D0.bin[kBinList];
+  int64_t K = len[0], nans = nan[0];
+  if (h->world > 1 && bin_world(h, len, nan, &curve, &K, &nans)) return 1;
+  CK(cudaSetDevice(D0.ordinal));
+  double areas[2] = {0.0, 0.0};
+  BinRec last = {0ull, 0, 0};
+  std::vector<BinRec> host;
+  if (K > 0) {
+    if (ensure_bin(h, D0, kBinTiles, 2 * (size_t)bin_area_blocks(K) * sizeof(double))) return 1;
+    double *dev_areas = (double *)((char *)D0.bin[kBinMisc] + kBinMiscAreas);
+    CK(bin_areas_launch(curve, K, (double *)D0.bin[kBinTiles], dev_areas, D0.st));
+    CK(cudaMemcpyAsync(areas, dev_areas, sizeof areas, cudaMemcpyDeviceToHost, D0.st));
+    CK(cudaMemcpyAsync(&last, curve + (K - 1), sizeof last, cudaMemcpyDeviceToHost, D0.st));
+    if (capacity >= K) {
+      host.resize((size_t)K);
+      CK(cudaMemcpyAsync(host.data(), curve, (size_t)K * sizeof(BinRec), cudaMemcpyDeviceToHost, D0.st));
+    }
+  }
+  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  const double nan_v = std::numeric_limits<double>::quiet_NaN();
+  const int64_t P = last.tp, Nn = last.fp;
+  out[AGD_BIN_POS] = (double)P;
+  out[AGD_BIN_NEG] = (double)Nn;
+  out[AGD_BIN_NAN] = (double)nans;
+  out[AGD_BIN_AUROC] = (P > 0 && Nn > 0) ? areas[0] : nan_v;
+  out[AGD_BIN_AUPR] = P > 0 ? areas[1] : nan_v;
+  *n_points = K;
+  for (size_t k = 0; k < host.size(); ++k) {
+    margin_out[k] = margin_of_key(host[k].key);
+    tp_out[k] = host[k].tp;
+    fp_out[k] = host[k].fp;
   }
   return 0;
 }

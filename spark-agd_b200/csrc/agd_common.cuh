@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/agd_b200.h"
 
@@ -103,8 +104,9 @@ struct XchgRs {
   unsigned int *ticket;
 };
 // The reduction the gather kernels apply to the W slots, in rank order: a sum, or a NaN-ignoring max (column maxima; a minimum
-// travels as the max of -x).  Either way every rank gets identical bits.
-enum { kXchgSum = 0, kXchgMax = 1 };
+// travels as the max of -x).  Either way every rank gets identical bits.  kXchgCopy is the concatenation of the W slots
+// (xchg_gather_copy_launch): no arithmetic touches the payload, so bit-cast keys and counts travel unchanged.
+enum { kXchgSum = 0, kXchgMax = 1, kXchgCopy = 2 };
 cudaError_t xchg_rs_publish_launch(const double *acc, const XchgRs &x, cudaStream_t st);
 cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st,
                                         int op = kXchgSum);
@@ -115,9 +117,19 @@ inline size_t xchg_rs_slice(int S, int W) { return ((size_t)S + W - 1) / W; }
 inline size_t xchg_off_rs(int S, int W) { return 2 * (size_t)W * S; }
 inline size_t xchg_off_res(int S, int W) { return xchg_off_rs(S, W) + 2 * (size_t)W * xchg_rs_slice(S, W); }
 inline size_t xchg_total_doubles(int S, int W) { return xchg_off_res(S, W) + 2 * (size_t)S; }
+// Bulk area behind the areas above, [2][W][kXchgBulk] doubles, for payloads that do not fit a slot (agd_binary_curve's lists):
+// the same publish kernel and flags with the peers' bases moved to xchg_off_bulk and a slot stride of kXchgBulk, one epoch per
+// chunk of at most kXchgBulk doubles.  It only extends the one allocation each rank exports, so no offset of the areas above
+// and no handle format changes.
+constexpr int kXchgBulk = 65536;
+inline size_t xchg_off_bulk(int S, int W) { return xchg_total_doubles(S, W); }
+inline size_t xchg_alloc_doubles(int S, int W) { return xchg_off_bulk(S, W) + 2 * (size_t)W * kXchgBulk; }
 cudaError_t xchg_publish_launch(const double *acc, const XchgPub &pub, cudaStream_t st);
 cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
                                int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st, int op = kXchgSum);
+// kXchgCopy: waits for the W flags like xchg_gather_launch, then out[r * out_stride + c] = slot r [c], c < n
+cudaError_t xchg_gather_copy_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
+                                    int slot_stride, unsigned long long epoch, double *out, size_t out_stride, cudaStream_t st);
 
 // out[c] = sum_b slabs[b][c] for c < n, n = D + 4 or 2 (D + 4) (gradient sums, loss sum, row count, loss sum and count at w2; fixed order =>
 // deterministic);
@@ -171,10 +183,21 @@ struct ScoreArgs {
   int64_t row0 = 0, rows = 0;
   int32_t d = 0;                    // stored row length (the handle's internal dimension)
   int32_t kind = 0;                 // AGD_GRAD_* (evaluation)
-  double threshold = 0.0;           // evaluation: confusion-count threshold
-  double *margins = nullptr;        // margins form: rows doubles
-  double *slabs = nullptr;          // evaluation form: [score_max_blocks][AGD_EVAL_N]
-  long long row_base = 0;           // evaluation form: global index of the shard's first row ...
+  // The key form's outputs share the words of fields it does not use, so the kernels' parameter block keeps its size (and the
+  // margins and evaluation forms their register allocation).
+  union {
+    double threshold = 0.0;         // evaluation: confusion-count threshold
+    unsigned int *counters;         // key form: [0] = keys written, [1] = NaN margins (zeroed by the caller)
+  };
+  union {
+    double *margins = nullptr;      // margins form: rows doubles
+    unsigned long long *keys;       // key form: margin_key of the kept rows' non-NaN margins, compacted, ...
+  };
+  union {
+    double *slabs = nullptr;        // evaluation form: [score_max_blocks][AGD_EVAL_N]
+    uint8_t *classes;               // key form: ... and their classes (1: label > 0.5)
+  };
+  long long row_base = 0;           // evaluation and key forms: global index of the shard's first row ...
   const RowFilter *filt = nullptr;  // ... and the view whose rows are summed (rows outside it are not even read)
   cudaStream_t stream = nullptr;
 };
@@ -182,6 +205,53 @@ int score_max_blocks(int sm_count);
 cudaError_t score_margins_launch(const ScoreArgs &a, int elem_bytes, int sm_count);
 // *blocks_out = slabs written (0 for an empty range)
 cudaError_t score_eval_launch(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out);
+cudaError_t score_keys_launch(const ScoreArgs &a, int elem_bytes, int sm_count);
+
+// ---------------------------------------------------------------- ranking metrics (rank.cu, agd_binary_curve)
+// The descending-order key of a non-NaN margin: the fp64 bits (-0 taken as +0) mapped to an unsigned integer whose ascending
+// order is the DESCENDING order of the margins (so a key sort puts the highest score first).  margin_of_key inverts it.
+__host__ __device__ inline unsigned long long margin_key(double m) {
+  if (m == 0.0) m = 0.0;
+  unsigned long long u;
+  memcpy(&u, &m, sizeof u);
+  const unsigned long long asc = (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+  return ~asc;
+}
+__host__ __device__ inline double margin_of_key(unsigned long long k) {
+  const unsigned long long asc = ~k;
+  const unsigned long long u = (asc >> 63) ? (asc & 0x7fffffffffffffffull) : ~asc;
+  double m;
+  memcpy(&m, &u, sizeof m);
+  return m;
+}
+// One point of the curve: a distinct key and the cumulative counts of positives / negatives down to it (inclusive).
+struct BinRec {
+  unsigned long long key;
+  long long tp, fp;
+};
+// Stable LSD radix sort of (key, value) pairs, 8-bit digits, value 1 byte (a class) or 4 bytes (an index).  keys[0] / vals[0]
+// hold the input; *which = the buffer pair holding the result.  One histogram of all eight digits decides the passes first:
+// a pass whose digit is the same in every key is skipped.  hist: 8 x 256 counters; tiles: bin_sort_tile_words(n) words.
+// Synchronises the stream once (the histogram decides the passes on the host).
+size_t bin_sort_tile_words(long long n);
+cudaError_t bin_sort_pairs(unsigned long long *keys[2], void *vals[2], int val_bytes, long long n, unsigned *hist,
+                           unsigned *tiles, int *which, int *passes, cudaStream_t st);
+// Run-length reduce of sorted pairs into the curve: out[r] = {key, cumulative positives, cumulative negatives} of the r-th
+// distinct key, *n_out = distinct keys.  val_bytes 1: vals are classes; 4: vals index (pos, neg) in upos / uneg.
+// tile_sums: bin_runs_tile_words(n) long longs.
+size_t bin_runs_tile_words(long long n);
+cudaError_t bin_runs_launch(const unsigned long long *keys, const void *vals, int val_bytes, const long long *upos,
+                            const long long *uneg, long long n, long long *tile_sums, BinRec *out, long long *n_out,
+                            cudaStream_t st);
+// The world's lists (rank r's records off[r + 1] - off[r] of them, at blocks + r * stride) concatenated in rank order: key,
+// index, and each record's own counts (the difference of consecutive cumulative counts within its list).  off: world + 1
+// offsets in device memory.
+cudaError_t bin_union_prep_launch(const BinRec *blocks, long long stride, const long long *off, int world, long long total,
+                                  unsigned long long *keys, uint32_t *idx, long long *upos, long long *uneg, cudaStream_t st);
+// Trapezoid areas under ROC and PR of the K-point curve (K >= 1): out[0] = AUROC, out[1] = AUPR, summed in a fixed order
+// (per block in index order, then the blocks in order).  partials: bin_area_blocks(K) x 2 doubles.
+int bin_area_blocks(long long K);
+cudaError_t bin_areas_launch(const BinRec *recs, long long K, double *partials, double *out, cudaStream_t st);
 // ---------------------------------------------------------------- column statistics (colstats.cu, agd_col_stats)
 // Pass 1 sums, per device and after the exchange: [SUM d | SQ d | ABS d | NNZ d | COUNT 1 | STORED d] (col_sum_n(d) doubles);
 // maxima [MAX d | -MIN d]; pass 2 sums [DEV d | DEV2 d].  STORED is the stored-entry count of a CSR column (= COUNT on

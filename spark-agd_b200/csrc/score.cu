@@ -15,7 +15,10 @@
 //     one slab per CTA; k1_reduce_launch then adds the slabs in a fixed order, so repeated calls return identical bits
 //     (also on CSR shards, where K1 scatters with RED.ADD).
 // Non-finite features follow IEEE arithmetic: nothing is skipped (0 * inf = NaN, as ddot gives).
-// On a view (agd_set_row_filter) the evaluation form treats a row outside it as past the end of the shard: its loads are
+//   * the key form (agd_binary_curve) writes, for every row of the view whose margin is not NaN, the 64-bit descending-order
+//     key of the margin (margin_key, agd_common.cuh) and the row's class (label > 0.5), compacted by one atomic per warp and
+//     step; NaN margins are only counted.  The margin is the G-lane margin above, so a key carries agd_margins' bits.
+// On a view (agd_set_row_filter) the evaluation and key forms treat a row outside it as past the end of the shard: its loads are
 // never issued, so it leaves no trace in the sums, and a held-out view reads only its own rows' lines of X.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -29,6 +32,7 @@ namespace agd {
 namespace {
 
 constexpr int kScoreThreads = 256;
+enum { kScoreMargins = 0, kScoreEval = 1, kScoreKeys = 2 };   // the three forms of the scoring sweeps
 constexpr int kCsrGroup = 8;                 // lanes per CSR row
 // w (fp64) lives in dynamic shared memory when it fits beside the evaluation form's static reduction array within the
 // 48 KB a block gets without an opt-in: up to d = 6056
@@ -127,11 +131,29 @@ __device__ __forceinline__ double group_sum(double v, int G) {
 // R rows per row group and step: one load of w serves R rows, and R rows of loads are in flight per lane
 template <typename T> struct ScoreRows { static constexpr int R = 4; };
 
-template <typename T, bool VEC, bool EVAL>
+// key form: every lane of the warp calls it (the row loops are warp-uniform); `ok` rows with a non-NaN margin are appended
+// to keys / classes, NaN margins are counted
+__device__ __forceinline__ void key_emit(const ScoreArgs &a, bool ok, double m, double y) {
+  const bool nan = ok && m != m, emit = ok && !nan;
+  const unsigned em = __ballot_sync(0xffffffffu, emit), nm = __ballot_sync(0xffffffffu, nan);
+  const int lane = threadIdx.x & 31;
+  unsigned base = 0;
+  if (lane == 0 && em) base = atomicAdd(a.counters, (unsigned)__popc(em));
+  if (lane == 0 && nm) atomicAdd(a.counters + 1, (unsigned)__popc(nm));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (emit) {
+    const unsigned i = base + __popc(em & ((1u << lane) - 1u));
+    a.keys[i] = margin_key(m);
+    a.classes[i] = y > 0.5 ? 1 : 0;
+  }
+}
+
+template <typename T, bool VEC, int MODE>
 __global__ void __launch_bounds__(kScoreThreads, 2) score_dense_kernel(const ScoreArgs a, const int G, const int w_smem) {
   extern __shared__ __align__(16) double w_sh[];
   constexpr int EPV = VEC ? ScoreElem<T>::EPV : 1;
   constexpr int R = ScoreRows<T>::R;
+  constexpr bool EVAL = MODE == kScoreEval, VIEWED = MODE != kScoreMargins;
   const int lane = threadIdx.x & 31;
   const double *w = a.w;
   if (w_smem) {
@@ -156,7 +178,7 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_dense_kernel(const Sco
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       row[r] = base + (long long)r * groups + g;
-      ok[r] = row[r] < a.rows && (!EVAL || row_in_view(a.filt, a.row_base + a.row0 + row[r]));
+      ok[r] = row[r] < a.rows && (!VIEWED || row_in_view(a.filt, a.row_base + a.row0 + row[r]));
       acc[r] = 0.0;
     }
     const T *xr[R];
@@ -164,7 +186,7 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_dense_kernel(const Sco
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       xr[r] = X + (size_t)(a.row0 + (ok[r] ? row[r] : 0)) * a.d;
-      yv[r] = (EVAL && ok[r]) ? __ldg(a.labels + a.row0 + row[r]) : 0.0;
+      yv[r] = (VIEWED && ok[r]) ? __ldg(a.labels + a.row0 + row[r]) : 0.0;
     }
 #pragma unroll 2
     for (int u = l; u < nunit; u += G) {
@@ -205,25 +227,35 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_dense_kernel(const Sco
 #pragma unroll
       for (int r = 1; r < R; ++r)
         if (l == r) { mm = m[r]; y = yv[r]; rr = row[r]; o = ok[r]; }
-      if (l < R && o) {
-        if (EVAL) eval_row(s, a.kind, a.threshold, mm, y);
-        else a.margins[rr] = mm;
+      if constexpr (MODE == kScoreKeys) {
+        key_emit(a, l < R && o, mm, y);
+      } else {
+        if (l < R && o) {
+          if (EVAL) eval_row(s, a.kind, a.threshold, mm, y);
+          else a.margins[rr] = mm;
+        }
       }
     } else {
 #pragma unroll
-      for (int r = 0; r < R; ++r)
-        if (ok[r] && l == 0) {
-          if (EVAL) eval_row(s, a.kind, a.threshold, m[r], yv[r]);
-          else a.margins[row[r]] = m[r];
+      for (int r = 0; r < R; ++r) {
+        if constexpr (MODE == kScoreKeys) {
+          key_emit(a, ok[r] && l == 0, m[r], yv[r]);
+        } else {
+          if (ok[r] && l == 0) {
+            if (EVAL) eval_row(s, a.kind, a.threshold, m[r], yv[r]);
+            else a.margins[row[r]] = m[r];
+          }
         }
+      }
     }
   }
   if (EVAL) eval_flush(s, a.slabs);
 }
 
-template <typename T, bool EVAL>
+template <typename T, int MODE>
 __global__ void __launch_bounds__(kScoreThreads) score_csr_kernel(const ScoreArgs a) {
   constexpr int G = kCsrGroup, groups = 32 / G;
+  constexpr bool EVAL = MODE == kScoreEval, VIEWED = MODE != kScoreMargins;
   const int lane = threadIdx.x & 31, g = lane / G, l = lane & (G - 1);
   const long long warp0 = (long long)blockIdx.x * (kScoreThreads / 32) + (threadIdx.x >> 5);
   const long long nwarps = (long long)gridDim.x * (kScoreThreads / 32);
@@ -233,7 +265,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_csr_kernel(const ScoreArg
   for (int k = 0; k < AGD_EVAL_N; ++k) s[k] = 0.0;
   for (long long base = warp0 * groups; base < a.rows; base += nwarps * groups) {
     const long long row = base + g;
-    const bool ok = row < a.rows && (!EVAL || row_in_view(a.filt, a.row_base + a.row0 + row));
+    const bool ok = row < a.rows && (!VIEWED || row_in_view(a.filt, a.row_base + a.row0 + row));
     double acc = 0.0;
     if (ok) {
       const long long r = a.row0 + row;
@@ -242,7 +274,8 @@ __global__ void __launch_bounds__(kScoreThreads) score_csr_kernel(const ScoreArg
       for (long long k = k0 + l; k < k1; k += G) acc = fma(ScoreElem<T>::one(val + k), __ldg(a.w + __ldg(a.idx + k)), acc);
     }
     const double m = group_sum(acc, G) + a.b;
-    if (ok && l == 0) {
+    if constexpr (MODE == kScoreKeys) key_emit(a, ok && l == 0, m, (ok && l == 0) ? a.labels[a.row0 + row] : 0.0);
+    else if (ok && l == 0) {
       if (EVAL) eval_row(s, a.kind, a.threshold, m, a.labels[a.row0 + row]);
       else a.margins[row] = m;
     }
@@ -265,7 +298,7 @@ cudaError_t persistent_grid(K kern, int smem, int sm_count, long long rows, long
   return cudaSuccess;
 }
 
-template <typename T, bool VEC, bool EVAL>
+template <typename T, bool VEC, int MODE>
 cudaError_t launch_dense(const ScoreArgs &a, int sm_count, int *blocks_out) {
   constexpr int EPV = VEC ? ScoreElem<T>::EPV : 1;
   const int nunit = a.d / EPV;
@@ -273,7 +306,7 @@ cudaError_t launch_dense(const ScoreArgs &a, int sm_count, int *blocks_out) {
   while (G < nunit && G < 32) G <<= 1;
   const int w_smem = a.d <= kScoreWSmemMax ? 1 : 0;
   const int smem = w_smem ? a.d * (int)sizeof(double) : 0;
-  auto kern = score_dense_kernel<T, VEC, EVAL>;
+  auto kern = score_dense_kernel<T, VEC, MODE>;
   int grid = 0;
   const cudaError_t e =
       persistent_grid(kern, smem, sm_count, a.rows, (long long)(kScoreThreads / 32) * (32 / G) * ScoreRows<T>::R, &grid);
@@ -283,19 +316,19 @@ cudaError_t launch_dense(const ScoreArgs &a, int sm_count, int *blocks_out) {
   return cudaGetLastError();
 }
 
-template <typename T, bool EVAL>
+template <typename T, int MODE>
 cudaError_t launch_dense_t(const ScoreArgs &a, int sm_count, int *blocks_out) {
-  if ((a.d * sizeof(T)) % 16 == 0) return launch_dense<T, true, EVAL>(a, sm_count, blocks_out);
-  return launch_dense<T, false, EVAL>(a, sm_count, blocks_out);
+  if ((a.d * sizeof(T)) % 16 == 0) return launch_dense<T, true, MODE>(a, sm_count, blocks_out);
+  return launch_dense<T, false, MODE>(a, sm_count, blocks_out);
 }
 
-template <bool EVAL>
+template <int MODE>
 cudaError_t launch_any(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out) {
   *blocks_out = 0;
   if (a.rows <= 0) return cudaSuccess;
   if (a.rowptr) {
     if (elem_bytes != 4 && elem_bytes != 8) return cudaErrorInvalidValue;
-    auto kern = elem_bytes == 8 ? score_csr_kernel<double, EVAL> : score_csr_kernel<float, EVAL>;
+    auto kern = elem_bytes == 8 ? score_csr_kernel<double, MODE> : score_csr_kernel<float, MODE>;
     int grid = 0;
     const cudaError_t e = persistent_grid(kern, 0, sm_count, a.rows, (long long)(kScoreThreads / 32) * (32 / kCsrGroup), &grid);
     if (e != cudaSuccess) return e;
@@ -303,9 +336,9 @@ cudaError_t launch_any(const ScoreArgs &a, int elem_bytes, int sm_count, int *bl
     kern<<<grid, kScoreThreads, 0, a.stream>>>(a);
     return cudaGetLastError();
   }
-  if (elem_bytes == 2) return launch_dense_t<__nv_bfloat16, EVAL>(a, sm_count, blocks_out);
-  if (elem_bytes == 4) return launch_dense_t<float, EVAL>(a, sm_count, blocks_out);
-  if (elem_bytes == 8) return launch_dense_t<double, EVAL>(a, sm_count, blocks_out);
+  if (elem_bytes == 2) return launch_dense_t<__nv_bfloat16, MODE>(a, sm_count, blocks_out);
+  if (elem_bytes == 4) return launch_dense_t<float, MODE>(a, sm_count, blocks_out);
+  if (elem_bytes == 8) return launch_dense_t<double, MODE>(a, sm_count, blocks_out);
   return cudaErrorInvalidValue;
 }
 
@@ -348,11 +381,16 @@ int score_max_blocks(int sm_count) { return 8 * sm_count; }
 
 cudaError_t score_margins_launch(const ScoreArgs &a, int elem_bytes, int sm_count) {
   int blocks = 0;
-  return launch_any<false>(a, elem_bytes, sm_count, &blocks);
+  return launch_any<kScoreMargins>(a, elem_bytes, sm_count, &blocks);
 }
 
 cudaError_t score_eval_launch(const ScoreArgs &a, int elem_bytes, int sm_count, int *blocks_out) {
-  return launch_any<true>(a, elem_bytes, sm_count, blocks_out);
+  return launch_any<kScoreEval>(a, elem_bytes, sm_count, blocks_out);
+}
+
+cudaError_t score_keys_launch(const ScoreArgs &a, int elem_bytes, int sm_count) {
+  int blocks = 0;
+  return launch_any<kScoreKeys>(a, elem_bytes, sm_count, &blocks);
 }
 
 }  // namespace agd

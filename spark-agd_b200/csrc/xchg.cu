@@ -60,6 +60,20 @@ __global__ void __launch_bounds__(256) xchg_gather_kernel(const double *xbuf, co
   }
 }
 
+// kXchgCopy: wait for the W flags of this epoch, then concatenate the W slots in rank order (plain moves: the bits travel)
+__global__ void __launch_bounds__(256) xchg_gather_copy_kernel(const double *xbuf, const unsigned long long *flags, int world,
+                                                               int buf, int n, int slot_stride, unsigned long long epoch,
+                                                               double *out, size_t out_stride) {
+  if (threadIdx.x < world) {
+    const volatile unsigned long long *f = flags + buf * world + threadIdx.x;
+    while (*f < epoch) __nanosleep(20);
+    __threadfence_system();
+  }
+  __syncthreads();
+  for (int c = blockIdx.x * 256 + threadIdx.x; c < n; c += gridDim.x * 256)
+    for (int r = 0; r < world; ++r) out[(size_t)r * out_stride + c] = __ldcg(xbuf + ((size_t)buf * world + r) * slot_stride + c);
+}
+
 // ---- reduce-scatter + all-gather for large payloads (see agd_common.cuh)
 // step 1: slice p of this rank's partial sums -> slot my_rank of rank p's rs area; then the "arrived" flag on every peer
 __global__ void __launch_bounds__(256) xchg_rs_publish_kernel(const double *__restrict__ acc, const XchgRs x) {
@@ -178,6 +192,15 @@ cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long lon
   if (grid > 64) grid = 64;
   if (op == kXchgMax) xchg_gather_kernel<kXchgMax><<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
   else xchg_gather_kernel<kXchgSum><<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, acc_out);
+  return cudaGetLastError();
+}
+
+cudaError_t xchg_gather_copy_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
+                                    int slot_stride, unsigned long long epoch, double *out, size_t out_stride, cudaStream_t st) {
+  int grid = (n + 255) / 256;
+  if (grid > 64) grid = 64;
+  if (grid < 1) grid = 1;
+  xchg_gather_copy_kernel<<<grid, 256, 0, st>>>(xbuf_local, flags_local, world, buf, n, slot_stride, epoch, out, out_stride);
   return cudaGetLastError();
 }
 

@@ -67,6 +67,11 @@ class _ThresholdModel(GeneralizedLinearModel):
             return score
         return (score > self.threshold).astype(np.float64)
 
+    def binaryMetrics(self, data: DeviceDataset, numBins: int = 0):
+        """BinaryClassificationMetrics of this model over every shard of `data` (a DeviceDataset or view; collective)."""
+        from .evaluation import BinaryClassificationMetrics
+        return BinaryClassificationMetrics(self, data, numBins)
+
     def _eval_threshold(self) -> float:
         # the confusion counts need a cut even when predict returns raw scores: the class default then
         return type(self).threshold if self.threshold is None else self.threshold

@@ -538,6 +538,27 @@ class DeviceDataset:
                                          _ptr(sums)), self.h)
         return Evaluation.from_sums(sums)
 
+    def binary_curve(self, w, intercept: float = 0.0, curve: bool = True):
+        """The ranking curve of the model (w, intercept) over every shard of the world (agd_binary_curve; collective: every
+        rank calls it, every rank gets the same bits): (summary, margins, tp, fp) with summary the AGD_BIN_N doubles [P, N,
+        NaN margins, areaUnderROC, areaUnderPR] and, with `curve`, the distinct margins in descending order and the cumulative
+        true / false positive counts down to each (None otherwise).  The curve costs a second call of the same kind (the
+        first one tells every rank its length)."""
+        w, intercept = self._physical_model(self._weights(w), intercept)
+        L = N.lib()
+        out = np.empty(N.BIN_N, dtype=np.float64)
+        k = C.c_int64()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(L.agd_binary_curve(self.h, _ptr(w), float(intercept), 0, None, None, None, C.byref(k), _ptr(out)), self.h)
+            if not curve:
+                return out, None, None, None
+            n = int(k.value)
+            m, tp, fp = np.empty(n), np.empty(n, dtype=np.int64), np.empty(n, dtype=np.int64)
+            N.check(L.agd_binary_curve(self.h, _ptr(w), float(intercept), n, _ptr(m) if n else None, _ptr(tp) if n else None,
+                                       _ptr(fp) if n else None, C.byref(k), _ptr(out)), self.h)
+        return out, m, tp, fp
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
