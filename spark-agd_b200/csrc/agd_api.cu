@@ -14,6 +14,7 @@
 #include <atomic>
 #include <chrono>
 #include <cmath>
+#include <functional>
 #include <limits>
 #include <mutex>
 #include <string>
@@ -142,6 +143,14 @@ struct Dev {
   std::vector<void *> xopened;            // cudaIpcOpenMemHandle mappings to close
 };
 
+// One epoch of the cross-rank exchange (open_epoch and the helpers around it)
+struct Epoch {
+  unsigned long long e = 0;   // 0: none (one rank, NCCL, or no exchange pending)
+  int n = 0;                  // doubles per rank
+  bool rs = false;            // reduce-scatter form (n >= kXchgRsMin)
+  bool bulk = false;          // through the bulk area, kXchgBulk doubles per slot
+};
+
 }  // namespace
 
 struct agd_handle {
@@ -171,11 +180,7 @@ struct agd_handle {
   int32_t x_d = 0;           // dimension the exchange buffers were built for (0 = not built)
   bool x_p2p = false;        // exchange buffers are live
   unsigned long long x_epoch = 0;
-  // a sweep whose gather was left to the K3 kernel that consumes it (smooth_device(..., defer_gather))
-  bool xg_pending = false;
-  bool xg_rs = false;        // the pending exchange is of the reduce-scatter form
-  unsigned long long xg_epoch = 0;
-  int xg_n = 0;
+  Epoch pending;             // a sweep whose gather was left to the K3 kernel that consumes it (smooth_device(..., defer_gather))
   std::string err;
   std::mutex mu;
   unsigned long long seq_base = 0;   // last round sequence number handed out (wait_scalars)
@@ -603,6 +608,134 @@ int ensure_xchg(agd_handle *h) {
   return 0;
 }
 
+// ---------------------------------------------------------------- the cross-rank exchange
+// Every payload that crosses ranks goes through the helpers below.  On the peer-memory exchange an epoch is one payload of at
+// most one slot (or one bulk chunk) per rank: every local device publishes, then every local device gathers, each in stream
+// order.  So a rank publishes epoch e + 2 only after its own gather of e + 1, which needed every rank's publish of e + 1, which
+// each rank enqueued after its gather of e: the parity buffer of e is free again when e + 2 writes into it.  (struct Epoch
+// is declared above agd_handle, which keeps the pending one.)
+// a buffer on local device i
+using DevBuf = std::function<double *(size_t i)>;
+
+Epoch open_epoch(agd_handle *h, int n, bool bulk = false) {
+  Epoch x;
+  if (h->world <= 1 || !h->x_p2p) return x;
+  x.e = ++h->x_epoch;
+  x.n = n;
+  x.rs = !bulk && n >= kXchgRsMin;
+  x.bulk = bulk;
+  return x;
+}
+
+// what local device i publishes in epoch x
+XchgPub publisher(const agd_handle *h, size_t i, const Epoch &x) {
+  const Dev &D = h->devs[i];
+  const int S = xchg_slot_stride(h->d), W = h->world;
+  XchgPub p;
+  p.peers = D.xpeers;
+  if (x.bulk)
+    for (int r = 0; r < W; ++r) p.peers.slot[r] += xchg_off_bulk(S, W);
+  p.world = W; p.my_rank = h->first_rank + (int)i; p.buf = (int)(x.e & 1ull); p.n = x.n;
+  p.slot_stride = x.bulk ? kXchgBulk : S;
+  p.epoch = x.e; p.ticket = D.xticket;
+  return p;
+}
+
+// what D gathers of epoch x: the slots (one-shot, bulk) or the finished sums (rs), and the flags that guard them; world == 0
+// when x is none
+XchgGather gatherer(const agd_handle *h, const Dev &D, const Epoch &x) {
+  XchgGather g;
+  if (!x.e) return g;
+  const int S = xchg_slot_stride(h->d), W = h->world;
+  g.xbuf = D.xbuf + (x.rs ? xchg_off_res(S, W) : x.bulk ? xchg_off_bulk(S, W) : 0);
+  g.flags = D.xflags + (x.rs ? xchg_flags_res(W) : xchg_flags_oneshot(W));
+  g.world = W; g.buf = (int)(x.e & 1ull); g.n = x.n;
+  g.slot_stride = x.bulk ? kXchgBulk : S;
+  g.rs = x.rs ? 1 : 0;
+  g.epoch = x.e;
+  return g;
+}
+
+// stand-alone publish of local device i's n doubles at src (the caller has made device i current): one-shot, or the rs publish
+// and the reduce-bcast of this rank's slice by op
+int publish(agd_handle *h, size_t i, const Epoch &x, const double *src, int op) {
+  const Dev &D = h->devs[i];
+  const XchgPub p = publisher(h, i, x);
+  if (x.rs) {
+    CK(xchg_rs_publish_launch(src, p, D.st));
+    CK(xchg_rs_reduce_bcast_launch(D.xbuf, D.xflags, p, D.st, op));
+  } else {
+    CK(xchg_publish_launch(src, p, D.st));
+  }
+  return 0;
+}
+
+// stand-alone gather of epoch x into dst(i) on every local device (see xchg_gather_launch)
+int gather(agd_handle *h, const Epoch &x, const DevBuf &dst, size_t out_stride, int op) {
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    CK(xchg_gather_launch(gatherer(h, D, x), dst(i), out_stride, op, D.st));
+  }
+  return 0;
+}
+
+// The NCCL form of an exchange (collective=nccl, or ranks that cannot map each other's memory): kXchgSum / kXchgMax all-reduce
+// the n doubles at buf(i) in place; kXchgCopy all-gathers rank r's n doubles at buf(i) into [W][n] at dst(i).
+int nccl_exchange(agd_handle *h, const DevBuf &buf, size_t n, int op, const DevBuf &dst = nullptr) {
+  if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
+  NcclApi &N = nccl_api();
+  CKN(N.GroupStart());
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    if (op == kXchgCopy) CKN(N.AllGather(buf(i), dst(i), n, ncclDouble, D.comm, D.st));   // moves bytes: no arithmetic
+    else CKN(N.AllReduce(buf(i), buf(i), n, ncclDouble, op == kXchgMax ? ncclMax : ncclSum, D.comm, D.st));
+  }
+  CKN(N.GroupEnd());
+  return 0;
+}
+
+// The all-reduce (sum, or NaN-ignoring max) of the n doubles at buf(i) on every local device: epochs of at most one slot
+// stride each (one-shot or reduce-scatter form by the epoch's size), or one NCCL all-reduce.
+int world_reduce(agd_handle *h, const DevBuf &buf, size_t n, int op) {
+  if (h->world <= 1 || n == 0) return 0;
+  if (!h->x_p2p) return nccl_exchange(h, buf, n, op);
+  const size_t S = (size_t)xchg_slot_stride(h->d);
+  for (size_t c0 = 0; c0 < n; c0 += S) {
+    const Epoch x = open_epoch(h, (int)std::min(S, n - c0));
+    for (size_t i = 0; i < h->devs.size(); ++i) {
+      CK(cudaSetDevice(h->devs[i].ordinal));
+      if (publish(h, i, x, buf(i) + c0, op)) return 1;
+    }
+    if (gather(h, x, [&](size_t i) { return buf(i) + c0; }, 0, op)) return 1;
+  }
+  return 0;
+}
+
+// Every rank's n doubles at src(i), concatenated in rank order into [W][n] at dst(i) on every local device: copy epochs
+// through the bulk area (one per kXchgBulk doubles), or one NCCL all-gather.
+int world_concat(agd_handle *h, const DevBuf &src, size_t n, const DevBuf &dst) {
+  if (!h->x_p2p) return nccl_exchange(h, src, n, kXchgCopy, dst);
+  for (size_t c0 = 0; c0 < n; c0 += kXchgBulk) {
+    const Epoch x = open_epoch(h, (int)std::min((size_t)kXchgBulk, n - c0), true);
+    for (size_t i = 0; i < h->devs.size(); ++i) {
+      CK(cudaSetDevice(h->devs[i].ordinal));
+      if (publish(h, i, x, src(i) + c0, kXchgCopy)) return 1;
+    }
+    if (gather(h, x, [&](size_t i) { return dst(i) + c0; }, n, kXchgCopy)) return 1;
+  }
+  return 0;
+}
+
+// drains every local stream
+int sync_all(agd_handle *h) {
+  for (Dev &D : h->devs) {
+    CK(cudaSetDevice(D.ordinal));
+    CK(cudaStreamSynchronize(D.st));
+  }
+  return 0;
+}
+
 void trace_mark(agd_handle *h, const char *tag) {
   if (h->trace < 0) { const char *e = getenv("AGD_TRACE"); h->trace = (e && *e && *e != '0') ? 1 : 0; }
   if (!h->trace) return;
@@ -676,28 +809,15 @@ bool dual_full_supported(const agd_handle *h) {
 // with dual_full also the gradient there -> a second block acc[D+4 .. 2D+7] = [grad | loss | count | 0 | 0].
 // D = h->model_d(): under a feature transform the points and the gradient are those of the model on appendBias(s o x);
 // K1 runs on the stored x at w_eff = (s o v, b) and the gradient columns are scaled by s before the exchange.
-// defer_gather: on the peer-memory path the gather is left to the next K3 kernel (h->xg_pending; see XchgGather) -- one launch
+// defer_gather: on the peer-memory path the gather is left to the next K3 kernel (h->pending; see XchgGather) -- one launch
 // fewer per sweep; the caller must hand the pending exchange to a k3_step / k3_gx launch before anything else reads acc.
 int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = nullptr, bool dual_full = false,
                   bool defer_gather = false) {
-  if (h->xg_pending) return fail(h, "internal: an exchange is still waiting for its consumer");
+  if (h->pending.e) return fail(h, "internal: an exchange is still waiting for its consumer");
   const int32_t d = h->d, md = h->model_d();
   const int32_t n = (dual_full ? 2 : 1) * (md + 4);   // doubles this sweep produces and exchanges
-  const bool p2p = h->world > 1 && h->x_p2p;
-  const bool rs = p2p && n >= kXchgRsMin;    // large payloads: reduce-scatter + all-gather instead of the one-shot exchange
-  const unsigned long long epoch = p2p ? ++h->x_epoch : 0ull;
-  auto make_rs = [&](Dev &D, size_t i) {
-    XchgRs x;
-    x.peers = D.xpeers; x.world = h->world; x.my_rank = h->first_rank + (int)i; x.buf = (int)(epoch & 1ull);
-    x.n = n; x.slot_stride = xchg_slot_stride(d); x.epoch = epoch; x.ticket = D.xticket;
-    return x;
-  };
-  auto make_pub = [&](Dev &D, size_t i) {
-    XchgPub pub;
-    pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
-    pub.n = n; pub.slot_stride = xchg_slot_stride(d); pub.epoch = epoch; pub.ticket = D.xticket;
-    return pub;
-  };
+  const Epoch ep = open_epoch(h, n);   // large payloads: reduce-scatter + all-gather instead of the one-shot exchange
+  const bool p2p = ep.e != 0, rs = ep.rs;
   for (size_t i = 0; i < h->devs.size(); ++i) {
     Dev &D = h->devs[i];
     CK(cudaSetDevice(D.ordinal));
@@ -725,11 +845,7 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
         CK(scale_columns_launch(D.acc, scale, d, D.st));
         if (i == 0) h->launches += 1;
       }
-      if (rs) {
-        const XchgRs x = make_rs(D, i);
-        CK(xchg_rs_publish_launch(D.acc, x, D.st));
-        CK(xchg_rs_reduce_bcast_launch(D.xbuf, D.xflags, x, D.st));
-      } else if (p2p) { const XchgPub pub = make_pub(D, i); CK(xchg_publish_launch(D.acc, pub, D.st)); }
+      if (p2p && publish(h, i, ep, D.acc, kXchgSum)) return 1;
       h->launches += (i == 0) ? (rs ? 4 : (p2p ? 3 : 2)) : 0;
       continue;
     }
@@ -764,43 +880,30 @@ int smooth_device(agd_handle *h, int kind, WSel w_of, bool timed, WSel w2_of = n
     else CK(k1_generic_launch(a, h->tf_bias, eb, D.sm_count, max_blocks, &blocks, D.st));
     if (t0) CK(cudaEventRecord(next_event(D.ev, D.ev_used), D.st));
     if (i == 0) trace_mark(h, dual_full ? "K1x2" : (w2_of ? "K1+loss" : "K1"));
-    if (p2p && !rs) { const XchgPub pub = make_pub(D, i); CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, &pub, D.st, scale, d, md + 4)); }
+    if (p2p && !rs) { const XchgPub pub = publisher(h, i, ep); CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, &pub, D.st, scale, d, md + 4)); }
     else CK(k1_reduce_launch(D.slabs, blocks, n, D.acc, nullptr, D.st, scale, d, md + 4));
     if (rs) {
-      const XchgRs x = make_rs(D, i);
-      CK(xchg_rs_publish_launch(D.acc, x, D.st));
-      CK(xchg_rs_reduce_bcast_launch(D.xbuf, D.xflags, x, D.st));
+      if (publish(h, i, ep, D.acc, kXchgSum)) return 1;
       if (i == 0) h->launches += 2;
     }
     if (i == 0) trace_mark(h, p2p ? "reduce+publish" : "reduce");
     if (i == 0) h->launches += (s.rows > 0 ? 2 : 1);
   }
+  const DevBuf acc = [h](size_t i) { return h->devs[i].acc; };
+  Dev &D0 = h->devs[0];
   if (p2p && defer_gather) {
-    h->xg_pending = true;
-    h->xg_rs = rs;
-    h->xg_epoch = epoch;
-    h->xg_n = n;
+    h->pending = ep;
     h->collectives += 1;
   } else if (p2p) {  // K2': every rank already holds every rank's partial sums; add them in rank order
-    Dev &D0 = h->devs[0];
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
-    for (Dev &D : h->devs) {
-      CK(cudaSetDevice(D.ordinal));
-      if (rs) CK(xchg_rs_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.acc, D.st));
-      else CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.acc, D.st));
-    }
+    if (gather(h, ep, acc, 0, kXchgSum)) return 1;
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
     trace_mark(h, "gather");
     h->launches += 1;
     h->collectives += 1;
   } else if (h->world > 1) {
-    if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
-    NcclApi &N = nccl_api();
-    Dev &D0 = h->devs[0];
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
-    CKN(N.GroupStart());
-    for (Dev &D : h->devs) CKN(N.AllReduce(D.acc, D.acc, (size_t)n, ncclDouble, ncclSum, D.comm, D.st));
-    CKN(N.GroupEnd());
+    if (nccl_exchange(h, acc, (size_t)n, kXchgSum)) return 1;
     if (timed) { CK(cudaSetDevice(D0.ordinal)); CK(cudaEventRecord(next_event(D0.ev_ar, D0.ev_ar_used), D0.st)); }
     h->collectives += 1;
   }
@@ -848,6 +951,7 @@ int sum_events(agd_handle *h, std::vector<cudaEvent_t> &pool, size_t used, doubl
 
 int check_ready(agd_handle *h) {
   if (!h) return 1;
+  h->pending = Epoch();   // a call that failed half-way may have left one behind
   if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
   for (Dev &D : h->devs)
     if (ensure_vectors(h, D, h->model_d())) return 1;
@@ -856,7 +960,6 @@ int check_ready(agd_handle *h) {
 }
 
 int call_begin(agd_handle *h) {
-  h->xg_pending = false;   // a call that failed half-way may have left one behind
   Dev &D = h->devs[0];
   CK(cudaSetDevice(D.ordinal));
   if (!h->ev_begin) { CK(cudaEventCreate(&h->ev_begin)); CK(cudaEventCreate(&h->ev_end)); }
@@ -872,7 +975,7 @@ int call_end(agd_handle *h, agd_stats &s, std::chrono::steady_clock::time_point 
   Dev &D0 = h->devs[0];
   CK(cudaSetDevice(D0.ordinal));
   CK(cudaEventRecord(h->ev_end, D0.st));
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, h->ev_begin, h->ev_end));
   s.device_ms_total = ms;
@@ -1275,7 +1378,7 @@ int agd_generate_csr(agd_handle *h, int64_t total_rows, int32_t d, int32_t nnz_p
     D.sh.rows = hi - lo;
     D.sh.nnz = (hi - lo) * nnz_per_row;
   }
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   return 0;
 }
 
@@ -1349,7 +1452,7 @@ int agd_generate(agd_handle *h, int64_t total_rows, int32_t d, int32_t store_dty
     CK(cudaMemsetAsync(D.wtmp, 0, ((size_t)di + 2) * sizeof(double), D.st));
     D.sh.rows = hi - lo;
   }
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   return 0;
 }
 
@@ -1443,7 +1546,6 @@ static int smooth_host(agd_handle *h, int32_t gradient, const double *w, const d
   }
   h->devs[0].ev_used = h->devs[0].ev_ar_used = 0;
   h->launches = h->collectives = 0;
-  h->xg_pending = false;
   if (smooth_device(h, gradient, [](Dev &D) { return (const double *)D.wtmp; }, false,
                     w2 ? (WSel)[](Dev &D) { return (const double *)D.g_x; } : (WSel) nullptr, grad2 != nullptr))
     return 1;
@@ -1451,7 +1553,7 @@ static int smooth_host(agd_handle *h, int32_t gradient, const double *w, const d
   CK(cudaSetDevice(D0.ordinal));
   std::vector<double> host(2 * ((size_t)d + 4));
   CK(cudaMemcpyAsync(host.data(), D0.acc, (grad2 ? 2 : 1) * ((size_t)d + 4) * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   const double cnt = host[(size_t)d + 1];
   *loss = host[d] / cnt;                                    // AGD.scala:207
   model_values(h, host.data(), cnt, grad);
@@ -1532,10 +1634,8 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
   if (check_ready(h)) return 1;
   if (gradient < 0 || gradient > AGD_GRAD_LEAST_SQUARES_HALF) return fail(h, "unknown gradient %d", gradient);
   if (!w || !out) return fail(h, "NULL argument");
-  h->xg_pending = false;
-  const int32_t d = h->d, n = AGD_EVAL_N;
-  const bool p2p = h->world > 1 && h->x_p2p;
-  const unsigned long long epoch = p2p ? ++h->x_epoch : 0ull;
+  const int32_t n = AGD_EVAL_N;
+  const Epoch ep = open_epoch(h, n);
   for (size_t i = 0; i < h->devs.size(); ++i) {
     Dev &D = h->devs[i];
     CK(cudaSetDevice(D.ordinal));
@@ -1547,31 +1647,23 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
     a.row_base = D.row_base; a.filt = h->filt_of(D);
     int blocks = 0;
     CK(score_eval_launch(a, D.sh.elem_bytes, D.sm_count, &blocks));
-    if (p2p) {
-      XchgPub pub;
-      pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
-      pub.n = n; pub.slot_stride = xchg_slot_stride(d); pub.epoch = epoch; pub.ticket = D.xticket;
+    if (ep.e) {
+      const XchgPub pub = publisher(h, i, ep);
       CK(k1_reduce_launch(D.slabs, blocks, n, D.eval, &pub, D.st));
     } else {
       CK(k1_reduce_launch(D.slabs, blocks, n, D.eval, nullptr, D.st));
     }
   }
-  if (p2p) {
-    for (Dev &D : h->devs) {
-      CK(cudaSetDevice(D.ordinal));
-      CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), n, xchg_slot_stride(d), epoch, D.eval, D.st));
-    }
+  const DevBuf eval = [h](size_t i) { return h->devs[i].eval; };
+  if (ep.e) {
+    if (gather(h, ep, eval, 0, kXchgSum)) return 1;
   } else if (h->world > 1) {
-    if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
-    NcclApi &N = nccl_api();
-    CKN(N.GroupStart());
-    for (Dev &D : h->devs) CKN(N.AllReduce(D.eval, D.eval, (size_t)n, ncclDouble, ncclSum, D.comm, D.st));
-    CKN(N.GroupEnd());
+    if (nccl_exchange(h, eval, (size_t)n, kXchgSum)) return 1;
   }
   Dev &D0 = h->devs[0];
   CK(cudaSetDevice(D0.ordinal));
   CK(cudaMemcpyAsync(out, D0.eval, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   return 0;
 }
 
@@ -1590,56 +1682,11 @@ static ColStatsLayout colstats_layout(int32_t d) {
   return L;
 }
 
-// The all-reduce of n doubles at D.cs + off on every local device (sum, or NaN-ignoring max): epochs of the peer-memory
-// exchange of at most one slot stride each (one-shot or reduce-scatter form by the epoch's size), or one NCCL all-reduce.
-static int colstats_allreduce(agd_handle *h, size_t off, size_t n, int op) {
-  if (h->world <= 1 || n == 0) return 0;
-  const int32_t d = h->d;
-  if (h->x_p2p) {
-    const size_t S = (size_t)xchg_slot_stride(d);
-    for (size_t c0 = 0; c0 < n; c0 += S) {
-      const int m = (int)(n - c0 < S ? n - c0 : S);
-      const bool rs = m >= kXchgRsMin;
-      const unsigned long long epoch = ++h->x_epoch;
-      for (size_t i = 0; i < h->devs.size(); ++i) {
-        Dev &D = h->devs[i];
-        CK(cudaSetDevice(D.ordinal));
-        if (rs) {
-          XchgRs x;
-          x.peers = D.xpeers; x.world = h->world; x.my_rank = h->first_rank + (int)i; x.buf = (int)(epoch & 1ull);
-          x.n = m; x.slot_stride = (int)S; x.epoch = epoch; x.ticket = D.xticket;
-          CK(xchg_rs_publish_launch(D.cs + off + c0, x, D.st));
-          CK(xchg_rs_reduce_bcast_launch(D.xbuf, D.xflags, x, D.st, op));
-        } else {
-          XchgPub pub;
-          pub.peers = D.xpeers; pub.world = h->world; pub.my_rank = h->first_rank + (int)i; pub.buf = (int)(epoch & 1ull);
-          pub.n = m; pub.slot_stride = (int)S; pub.epoch = epoch; pub.ticket = D.xticket;
-          CK(xchg_publish_launch(D.cs + off + c0, pub, D.st));
-        }
-      }
-      for (Dev &D : h->devs) {
-        CK(cudaSetDevice(D.ordinal));
-        if (rs) CK(xchg_rs_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), m, (int)S, epoch, D.cs + off + c0, D.st));
-        else CK(xchg_gather_launch(D.xbuf, D.xflags, h->world, (int)(epoch & 1ull), m, (int)S, epoch, D.cs + off + c0, D.st, op));
-      }
-    }
-    return 0;
-  }
-  if (!h->comm_ready || !h->devs[0].comm) return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", h->world);
-  NcclApi &N = nccl_api();
-  CKN(N.GroupStart());
-  for (Dev &D : h->devs)
-    CKN(N.AllReduce(D.cs + off, D.cs + off, n, ncclDouble, op == kXchgMax ? ncclMax : ncclSum, D.comm, D.st));
-  CKN(N.GroupEnd());
-  return 0;
-}
-
 // Collective: pass 1 on every local shard, the exchange of its sums and maxima, pass 2 (mu from the exchanged sums, on the
 // device), the exchange of its sums; the host then adds a CSR column's implicit zeros in closed form.
 int agd_col_stats(agd_handle *h, double *count, double *out) {
   if (check_ready(h)) return 1;
   if (!count || !out) return fail(h, "NULL argument");
-  h->xg_pending = false;
   const int32_t d = h->d, du = h->d_user;
   const ColStatsLayout L = colstats_layout(d);
   const size_t nsum1 = 4 * (size_t)d + 1;   // what a dense sweep's slabs carry of the pass-1 sums (STORED is filled after)
@@ -1674,8 +1721,8 @@ int agd_col_stats(agd_handle *h, double *count, double *out) {
       CK(colstats_fill_stored_launch(D.cs + L.sums, d, D.st));
     }
   }
-  if (colstats_allreduce(h, L.sums, col_sum_n(d), kXchgSum)) return 1;
-  if (colstats_allreduce(h, L.max, 2 * (size_t)d, kXchgMax)) return 1;
+  if (world_reduce(h, [&](size_t i) { return h->devs[i].cs + L.sums; }, col_sum_n(d), kXchgSum)) return 1;
+  if (world_reduce(h, [&](size_t i) { return h->devs[i].cs + L.max; }, 2 * (size_t)d, kXchgMax)) return 1;
   for (size_t i = 0; i < h->devs.size(); ++i) {
     Dev &D = h->devs[i];
     CK(cudaSetDevice(D.ordinal));
@@ -1694,12 +1741,12 @@ int agd_col_stats(agd_handle *h, double *count, double *out) {
       CK(k1_reduce_launch(a.slabs, blocks, 2 * d, D.cs + L.dev, nullptr, D.st));
     }
   }
-  if (colstats_allreduce(h, L.dev, 2 * (size_t)d, kXchgSum)) return 1;
+  if (world_reduce(h, [&](size_t i) { return h->devs[i].cs + L.dev; }, 2 * (size_t)d, kXchgSum)) return 1;
   Dev &D0 = h->devs[0];
   CK(cudaSetDevice(D0.ordinal));
   std::vector<double> r(L.keys);
   CK(cudaMemcpyAsync(r.data(), D0.cs, L.keys * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   const double n = r[4 * (size_t)d];
   *count = n;
   for (int32_t c = 0; c < du; ++c) {
@@ -1758,51 +1805,27 @@ static int bin_local(agd_handle *h, Dev &D, double intercept, int64_t *len, int6
   return 0;
 }
 
-// Every rank's list -> the world's curve on device 0 (*curve, *K records), identical on every rank: the lengths travel first
-// (a copy epoch of the exchange, or an NCCL all-gather), then the lists (rank r's at r * Lmax in kBinUnion: copy epochs through
-// the exchange's bulk area, or one all-gather); device 0 concatenates them in rank order, sorts and reduces again.
+// Every rank's list -> the world's curve on device 0 (*curve, *K records), identical on every rank: the lengths travel first,
+// then the lists (rank r's at r * Lmax in kBinUnion), each by world_concat; device 0 concatenates them in rank order, sorts and
+// reduces again.
 static int bin_world(agd_handle *h, const std::vector<int64_t> &len, const std::vector<int64_t> &nan, BinRec **curve,
                      int64_t *K, int64_t *nan_total) {
   const int W = h->world, nd = (int)h->devs.size();
-  const bool p2p = h->x_p2p;
-  const int S = xchg_slot_stride(h->d);
-  NcclApi &N = nccl_api();
-  if (!p2p && (!h->comm_ready || !h->devs[0].comm))
-    return fail(h, "world_ranks=%d but there is no communicator (agd_comm_init)", W);
   // 1. {list length, NaN count} of every rank
-  const unsigned long long e0 = p2p ? ++h->x_epoch : 0ull;
+  auto misc_at = [h](size_t i, size_t off) { return (double *)((char *)h->devs[i].bin[kBinMisc] + off); };
   for (int i = 0; i < nd; ++i) {
     Dev &D = h->devs[i];
     CK(cudaSetDevice(D.ordinal));
-    double *own = (double *)((char *)D.bin[kBinMisc] + kBinMiscOwn);
     const double v[2] = {(double)len[i], (double)nan[i]};
-    CK(cudaMemcpyAsync(own, v, sizeof v, cudaMemcpyHostToDevice, D.st));
+    CK(cudaMemcpyAsync(misc_at(i, kBinMiscOwn), v, sizeof v, cudaMemcpyHostToDevice, D.st));
     CK(cudaStreamSynchronize(D.st));   // v is on this stack frame
-    if (p2p) {
-      XchgPub pub;
-      pub.peers = D.xpeers; pub.world = W; pub.my_rank = h->first_rank + i; pub.buf = (int)(e0 & 1ull);
-      pub.n = 2; pub.slot_stride = S; pub.epoch = e0; pub.ticket = D.xticket;
-      CK(xchg_publish_launch(own, pub, D.st));
-    }
   }
-  if (p2p) {
-    for (Dev &D : h->devs) {
-      CK(cudaSetDevice(D.ordinal));
-      CK(xchg_gather_copy_launch(D.xbuf, D.xflags, W, (int)(e0 & 1ull), 2, S, e0, (double *)((char *)D.bin[kBinMisc] + kBinMiscAll), 2, D.st));
-    }
-  } else {
-    CKN(N.GroupStart());
-    for (Dev &D : h->devs) {
-      char *misc = (char *)D.bin[kBinMisc];
-      CKN(N.AllGather(misc + kBinMiscOwn, misc + kBinMiscAll, 2, ncclDouble, D.comm, D.st));
-    }
-    CKN(N.GroupEnd());
-  }
+  if (world_concat(h, [&](size_t i) { return misc_at(i, kBinMiscOwn); }, 2, [&](size_t i) { return misc_at(i, kBinMiscAll); })) return 1;
   std::vector<double> all((size_t)2 * W);
   Dev &D0 = h->devs[0];
   CK(cudaSetDevice(D0.ordinal));
-  CK(cudaMemcpyAsync(all.data(), (char *)D0.bin[kBinMisc] + kBinMiscAll, all.size() * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  CK(cudaMemcpyAsync(all.data(), misc_at(0, kBinMiscAll), all.size() * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
   std::vector<long long> off((size_t)W + 1, 0);
   long long lmax = 0, nans = 0;
   for (int r = 0; r < W; ++r) {
@@ -1818,43 +1841,15 @@ static int bin_world(agd_handle *h, const std::vector<int64_t> &len, const std::
   if (T >= (long long)1 << 31) return fail(h, "agd_binary_curve: %lld distinct scores over the world (at most 2^31 - 1)", T);
   // 2. the lists
   const size_t ld = 3 * (size_t)lmax;   // doubles of one rank's block
+  auto uni = [h](size_t i) { return (double *)h->devs[i].bin[kBinUnion]; };
   for (int i = 0; i < nd; ++i) {
     Dev &D = h->devs[i];
     CK(cudaSetDevice(D.ordinal));
     if (ensure_bin(h, D, kBinUnion, (size_t)W * ld * sizeof(double))) return 1;
-    double *mine = (double *)D.bin[kBinUnion] + (size_t)(h->first_rank + i) * ld;
-    if (len[i] > 0) CK(cudaMemcpyAsync(mine, D.bin[kBinList], (size_t)len[i] * sizeof(BinRec), cudaMemcpyDeviceToDevice, D.st));
+    if (len[i] > 0) CK(cudaMemcpyAsync(uni(i) + (size_t)(h->first_rank + i) * ld, D.bin[kBinList], (size_t)len[i] * sizeof(BinRec),
+                                       cudaMemcpyDeviceToDevice, D.st));
   }
-  if (p2p) {
-    const size_t off_bulk = xchg_off_bulk(S, W);
-    for (size_t c0 = 0; c0 < ld; c0 += kXchgBulk) {
-      const int m = (int)std::min((size_t)kXchgBulk, ld - c0);
-      const unsigned long long e = ++h->x_epoch;
-      for (int i = 0; i < nd; ++i) {
-        Dev &D = h->devs[i];
-        CK(cudaSetDevice(D.ordinal));
-        XchgPub pub;
-        pub.peers = D.xpeers;
-        for (int r = 0; r < W; ++r) pub.peers.slot[r] += off_bulk;
-        pub.world = W; pub.my_rank = h->first_rank + i; pub.buf = (int)(e & 1ull);
-        pub.n = m; pub.slot_stride = kXchgBulk; pub.epoch = e; pub.ticket = D.xticket;
-        CK(xchg_publish_launch((double *)D.bin[kBinUnion] + (size_t)pub.my_rank * ld + c0, pub, D.st));
-      }
-      for (Dev &D : h->devs) {
-        CK(cudaSetDevice(D.ordinal));
-        CK(xchg_gather_copy_launch(D.xbuf + off_bulk, D.xflags, W, (int)(e & 1ull), m, kXchgBulk, e, (double *)D.bin[kBinUnion] + c0,
-                                   ld, D.st));
-      }
-    }
-  } else {
-    CKN(N.GroupStart());
-    for (int i = 0; i < nd; ++i) {
-      Dev &D = h->devs[i];
-      double *u = (double *)D.bin[kBinUnion];
-      CKN(N.AllGather(u + (size_t)(h->first_rank + i) * ld, u, ld, ncclDouble, D.comm, D.st));   // moves bytes: no arithmetic
-    }
-    CKN(N.GroupEnd());
-  }
+  if (world_concat(h, [&](size_t i) { return uni(i) + (size_t)(h->first_rank + (int)i) * ld; }, ld, uni)) return 1;
   // 3. device 0: the concatenation in rank order, sorted and reduced
   CK(cudaSetDevice(D0.ordinal));
   const size_t t1 = (size_t)T;
@@ -1890,7 +1885,6 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
   if (!w || !n_points || !out) return fail(h, "NULL argument");
   if (capacity < 0) return fail(h, "capacity must be >= 0 (got %lld)", (long long)capacity);
   if (capacity > 0 && (!margin_out || !tp_out || !fp_out)) return fail(h, "NULL argument");
-  h->xg_pending = false;
   const int nd = (int)h->devs.size();
   std::vector<int64_t> len((size_t)nd), nan((size_t)nd);
   for (int i = 0; i < nd; ++i) {
@@ -1918,7 +1912,7 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
       CK(cudaMemcpyAsync(host.data(), curve, (size_t)K * sizeof(BinRec), cudaMemcpyDeviceToHost, D0.st));
     }
   }
-  for (Dev &D : h->devs) { CK(cudaSetDevice(D.ordinal)); CK(cudaStreamSynchronize(D.st)); }
+  if (sync_all(h)) return 1;
   const double nan_v = std::numeric_limits<double>::quiet_NaN();
   const int64_t P = last.tp, Nn = last.fp;
   out[AGD_BIN_POS] = (double)P;
@@ -2121,18 +2115,6 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
     CK(cudaHostAlloc(&H0.hist_host, H0.hist_cap * sizeof(double), cudaHostAllocMapped | cudaHostAllocPortable));
     CK(cudaHostGetDevicePointer((void **)&H0.hist_dev, H0.hist_host, 0));
   }
-  // the gather of a sweep is done by the K3 kernel that consumes its sums (one launch fewer per sweep)
-  auto take_gather = [&](Dev &D) {
-    XchgGather g;
-    if (h->xg_pending) {
-      const int S = xchg_slot_stride(h->d), W = h->world;
-      g.world = W; g.buf = (int)(h->xg_epoch & 1ull); g.n = h->xg_n; g.slot_stride = S; g.epoch = h->xg_epoch;
-      g.rs = h->xg_rs ? 1 : 0;
-      g.xbuf = h->xg_rs ? D.xbuf + xchg_off_res(S, W) : D.xbuf;       // rs: the area of finished sums
-      g.flags = h->xg_rs ? D.xflags + 4 * W : D.xflags;               // rs: the "finished slice arrived" flags
-    }
-    return g;
-  };
   long long pending_hist = -1;        // slot of H0.hist_host the next k3_step fills from the fused sweep it consumes
   std::vector<double> cx_of;          // c_x per iteration (:305)
   std::vector<char> fx_deferred;      // f_x of iteration k still sits in H0.hist_host[2k..2k+1]
@@ -2173,11 +2155,11 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
             a.partials = D.partials; a.ticket = D.ticket; a.scalars = D.scalars_dev;
             a.theta = theta; a.one_minus_theta = omt; a.step = step; a.reg = p->reg_param; a.d = d; a.updater = p->updater;
             if (!speculate) { a.seq_out = reinterpret_cast<unsigned long long *>(D.scalars_dev + 2 * K3_NS); a.seq = round_seq + 1; }
-            a.xg = take_gather(D); a.acc_w = D.acc;
+            a.xg = gatherer(h, D, h->pending); a.acc_w = D.acc;   // the K3 kernel gathers the sweep it consumes
             a.hist_out = (pending_hist >= 0 && &D == &h->devs[0]) ? D.hist_dev + pending_hist : nullptr;
             return k3_step_launch(a, D.st);
           })) return 1;
-      h->xg_pending = false;
+      h->pending = Epoch();
       pending_hist = -1;
       if (speculate) {                                                     // :269, enqueued before :265 is known
         if (guessed) {
@@ -2190,10 +2172,10 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
               a.acc = D.acc; a.x = D.x; a.y = D.y; a.g_y = D.g_y; a.g_x = D.g_x; a.partials = D.partials;
               a.ticket = D.ticket; a.scalars = D.scalars_dev + K3_NS; a.d = d;
               a.seq_out = reinterpret_cast<unsigned long long *>(D.scalars_dev + 2 * K3_NS); a.seq = round_seq + 1;
-              a.xg = take_gather(D); a.acc_w = D.acc;
+              a.xg = gatherer(h, D, h->pending); a.acc_w = D.acc;
               return k3_gx_launch(a, D.st);
             })) return 1;
-        h->xg_pending = false;
+        h->pending = Epoch();
       }
       if (wait_scalars(h, ++round_seq, sc)) return 1;                      // the one host wait of this round (no stream drain)
       trace_mark(h, "host-gap");
@@ -2299,7 +2281,7 @@ int agd_run(agd_handle *h, const agd_params *p, const double *w0, double *w_out,
     CK(cudaSetDevice(D.ordinal));
     if (get_point(h, D, w_out, D.x)) return 1;                             // :337
   }
-  if (h->xg_pending || pending_hist >= 0) return fail(h, "internal: a sweep was left without its consumer");
+  if (h->pending.e || pending_hist >= 0) return fail(h, "internal: a sweep was left without its consumer");
   if (call_end(h, s, t_begin)) return 1;
   trace_report(h, memoize ? "agd_run memoised" : (fuse ? "agd_run" : "agd_run unfused"));
   for (int k = 0; k < nh; ++k)                                             // :306 for the deferred f_x values

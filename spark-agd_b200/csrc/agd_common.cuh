@@ -71,10 +71,11 @@ struct XchgPeers {
   double *slot[kMaxRanks];               // base of rank p's xbuf as mapped into THIS device
   unsigned long long *flag[kMaxRanks];   // base of rank p's flags
 };
+// The publish half of one epoch on one rank, in the one-shot or the reduce-scatter form (below).
 struct XchgPub {
   XchgPeers peers;
   int world, my_rank, buf, n;
-  int slot_stride;          // doubles between two ranks' slots: xchg_slot_stride(d), the buffers' capacity per slot, NOT this
+  int slot_stride;          // doubles between two ranks' slots: xchg_slot_stride(d) (kXchgBulk in the bulk area), the capacity, NOT this
                             // sweep's n: sweeps of different payloads -- d + 4, 2 (d + 4) or AGD_EVAL_N -- must not move the
                             // slots of the other parity buffer
   unsigned long long epoch;
@@ -84,7 +85,7 @@ struct XchgPub {
 // the consumer waits for the W flags, adds the W slots in rank order where it needs a value, and writes every one of the n sums
 // to `acc` for later readers.  world == 0: nothing pending, read `acc` as usual.
 struct XchgGather {
-  const double *xbuf = nullptr;               // this device's exchange buffer [2][W][slot_stride] (one-shot) or its result area (rs)
+  const double *xbuf = nullptr;               // this device's [2][W][slot_stride] slots (one-shot or bulk area) or its result area (rs)
   const unsigned long long *flags = nullptr;  // [2][W] of the flag set to wait on
   int world = 0, buf = 0, n = 0, slot_stride = 0;
   int rs = 0;                                 // 1: reduce-scatter form -- the finished sums sit at xbuf[buf * slot_stride + j]
@@ -94,42 +95,35 @@ struct XchgGather {
 // Rank r stores slice p of its partial sums into rank p's `rs` area (slot r), rank p adds the W slots of ITS slice in rank order
 // and stores the finished slice into every rank's `res` area; 2 n / W doubles leave each rank per sweep instead of n W.
 // Layout of one device's exchange allocation (doubles): [one-shot: 2 W S][rs: 2 W L][res: 2 S], S = xchg_slot_stride(d) (below), L = ceil(S / W);
-// flags (u64): [one-shot 2 W][rs arrived 2 W][res arrived 2 W].
+// flags (u64): [one-shot 2 W][rs arrived 2 W][res arrived 2 W].  The helpers below are the only place this layout is written.
 constexpr int kXchgRsMin = 32768;
-struct XchgRs {
-  XchgPeers peers;
-  int world, my_rank, buf, n;
-  int slot_stride;              // S
-  unsigned long long epoch;
-  unsigned int *ticket;
-};
-// The reduction the gather kernels apply to the W slots, in rank order: a sum, or a NaN-ignoring max (column maxima; a minimum
-// travels as the max of -x).  Either way every rank gets identical bits.  kXchgCopy is the concatenation of the W slots
-// (xchg_gather_copy_launch): no arithmetic touches the payload, so bit-cast keys and counts travel unchanged.
-enum { kXchgSum = 0, kXchgMax = 1, kXchgCopy = 2 };
-cudaError_t xchg_rs_publish_launch(const double *acc, const XchgRs &x, cudaStream_t st);
-cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgRs &x, cudaStream_t st,
-                                        int op = kXchgSum);
-// waits for the W finished slices and copies them to acc_out (stand-alone form of the rs gather)
-cudaError_t xchg_rs_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
-                                  int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st);
-inline size_t xchg_rs_slice(int S, int W) { return ((size_t)S + W - 1) / W; }
-inline size_t xchg_off_rs(int S, int W) { return 2 * (size_t)W * S; }
-inline size_t xchg_off_res(int S, int W) { return xchg_off_rs(S, W) + 2 * (size_t)W * xchg_rs_slice(S, W); }
-inline size_t xchg_total_doubles(int S, int W) { return xchg_off_res(S, W) + 2 * (size_t)S; }
+__host__ __device__ inline size_t xchg_rs_slice(int S, int W) { return ((size_t)S + W - 1) / W; }
+__host__ __device__ inline size_t xchg_off_rs(int S, int W) { return 2 * (size_t)W * S; }
+__host__ __device__ inline size_t xchg_off_res(int S, int W) { return xchg_off_rs(S, W) + 2 * (size_t)W * xchg_rs_slice(S, W); }
+__host__ __device__ inline size_t xchg_total_doubles(int S, int W) { return xchg_off_res(S, W) + 2 * (size_t)S; }
+__host__ __device__ inline int xchg_flags_oneshot(int) { return 0; }         // raised by a one-shot (or bulk) publish
+__host__ __device__ inline int xchg_flags_rs(int W) { return 2 * W; }        // a rank's slices arrived in the rs area
+__host__ __device__ inline int xchg_flags_res(int W) { return 4 * W; }       // a finished slice arrived in the res area
 // Bulk area behind the areas above, [2][W][kXchgBulk] doubles, for payloads that do not fit a slot (agd_binary_curve's lists):
 // the same publish kernel and flags with the peers' bases moved to xchg_off_bulk and a slot stride of kXchgBulk, one epoch per
 // chunk of at most kXchgBulk doubles.  It only extends the one allocation each rank exports, so no offset of the areas above
 // and no handle format changes.
 constexpr int kXchgBulk = 65536;
-inline size_t xchg_off_bulk(int S, int W) { return xchg_total_doubles(S, W); }
-inline size_t xchg_alloc_doubles(int S, int W) { return xchg_off_bulk(S, W) + 2 * (size_t)W * kXchgBulk; }
+__host__ __device__ inline size_t xchg_off_bulk(int S, int W) { return xchg_total_doubles(S, W); }
+__host__ __device__ inline size_t xchg_alloc_doubles(int S, int W) { return xchg_off_bulk(S, W) + 2 * (size_t)W * kXchgBulk; }
+// The reduction the gather kernels apply to the W slots, in rank order: a sum, or a NaN-ignoring max (column maxima; a minimum
+// travels as the max of -x).  Either way every rank gets identical bits.  kXchgCopy is the concatenation of the W slots: no
+// arithmetic touches the payload, so bit-cast keys and counts travel unchanged.
+enum { kXchgSum = 0, kXchgMax = 1, kXchgCopy = 2 };
 cudaError_t xchg_publish_launch(const double *acc, const XchgPub &pub, cudaStream_t st);
-cudaError_t xchg_gather_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
-                               int slot_stride, unsigned long long epoch, double *acc_out, cudaStream_t st, int op = kXchgSum);
-// kXchgCopy: waits for the W flags like xchg_gather_launch, then out[r * out_stride + c] = slot r [c], c < n
-cudaError_t xchg_gather_copy_launch(const double *xbuf_local, const unsigned long long *flags_local, int world, int buf, int n,
-                                    int slot_stride, unsigned long long epoch, double *out, size_t out_stride, cudaStream_t st);
+cudaError_t xchg_rs_publish_launch(const double *acc, const XchgPub &x, cudaStream_t st);
+cudaError_t xchg_rs_reduce_bcast_launch(const double *xbuf_local, const unsigned long long *flags_local, const XchgPub &x, cudaStream_t st,
+                                        int op);
+// The stand-alone gather (K3 kernels inline it): waits for the W flags of g's epoch, then
+//   op == kXchgCopy: out[r * out_stride + c] = slot r [c], c < n;
+//   g.rs:            out[c] = the finished sum c;
+//   otherwise:       out[c] = the W slots reduced by op in rank order.
+cudaError_t xchg_gather_launch(const XchgGather &g, double *out, size_t out_stride, int op, cudaStream_t st);
 
 // out[c] = sum_b slabs[b][c] for c < n, n = D + 4 or 2 (D + 4) (gradient sums, loss sum, row count, loss sum and count at w2; fixed order =>
 // deterministic);

@@ -2,10 +2,7 @@
 host-shipped CUDA IPC exchange.  Every rank gets the same bits, and on the whole data they equal a single-process run over the
 same rows; the
 dense lists span several chunks of the exchange's bulk area.  Collective calls after a curve keep their bits."""
-import json
 import os
-import socket
-import subprocess
 import sys
 
 import numpy as np
@@ -13,41 +10,15 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from rank_world import run_world  # noqa: E402
 import binmetrics_reference as R  # noqa: E402
 from binmetrics_worker import B, dense_data  # noqa: E402
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(world, out, timeout=600):
-    port = _free_port()
-    env = dict(os.environ, OMP_NUM_THREADS="1")
-    procs = [subprocess.Popen([sys.executable, os.path.join(HERE, "binmetrics_worker.py"), str(r), str(world), str(port), "0",
-                               out], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT) for r in range(world)]
-    logs, failed = [], False
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            failed = True
-            for q in procs:          # exactly the PIDs this test started
-                q.kill()
-            o, _ = p.communicate()
-        logs.append(o.decode(errors="replace")[-3000:])
-        failed = failed or p.returncode != 0
-    assert not failed, "a rank failed or hung:\n" + "\n-----\n".join(logs)
-    with open(out) as f:
-        return json.load(f)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 3])
 def test_binary_curve_world_over_ipc(tmp_path, world):
-    res = _spawn(world, str(tmp_path / "res.json"))
+    res = run_world("binmetrics_worker.py", world, str(tmp_path / "res.json"), timeout=600)
     assert len(res) == world
     for r in range(world):
         assert res[r]["curves"] == res[0]["curves"], r

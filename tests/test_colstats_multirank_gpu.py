@@ -1,10 +1,7 @@
 """Statistics.colStats in a process-per-rank world (tests/colstats_worker.py): worlds of 2 and 3 processes share one GPU over
 the host-shipped CUDA IPC exchange.  Every rank gets identical bits, they match the whole world's reference within the
 bounds of tests/test_colstats_gpu.py, and collective calls after colStats keep their bits."""
-import json
 import os
-import socket
-import subprocess
 import sys
 
 import numpy as np
@@ -12,35 +9,9 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from rank_world import run_world  # noqa: E402
 from colstats_worker import FIELDS, N_CSR, N_DENSE, csr_data, dense_data, rows_of  # noqa: E402
 from test_colstats_gpu import check_summary, csr_cols, dense_cols  # noqa: E402
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(world, out, timeout=600):
-    port = _free_port()
-    env = dict(os.environ, OMP_NUM_THREADS="1")
-    procs = [subprocess.Popen([sys.executable, os.path.join(HERE, "colstats_worker.py"), str(r), str(world), str(port), "0",
-                               out], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT) for r in range(world)]
-    logs, failed = [], False
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            failed = True
-            for q in procs:          # exactly the PIDs this test started
-                q.kill()
-            o, _ = p.communicate()
-        logs.append(o.decode(errors="replace")[-3000:])
-        failed = failed or p.returncode != 0
-    assert not failed, "a rank failed or hung:\n" + "\n-----\n".join(logs)
-    with open(out) as f:
-        return json.load(f)
 
 
 class _Summary:
@@ -57,7 +28,7 @@ class _Summary:
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 3])
 def test_colstats_world_over_ipc(tmp_path, world):
-    res = _spawn(world, str(tmp_path / "res.json"))
+    res = run_world("colstats_worker.py", world, str(tmp_path / "res.json"), timeout=600)
     assert len(res) == world
     for key in ("dense", "dense_view", "dense_again", "csr", "csr_view", "csr_cols"):
         assert all(rr[key] == res[0][key] for rr in res), key                 # identical bits on every rank

@@ -5,10 +5,7 @@ One PROCESS per rank, as under torchrun / one Spark executor per GPU.  On a box 
 device 0: the exchange buffers are then mapped through CUDA IPC on the same device and the handles travel through the
 host (transport="ipc", no NCCL -- NCCL refuses two ranks on one GPU), so the IPC + epoch-flag protocol is exercised
 even where only one GPU exists.  With two or more GPUs the same worlds also run one rank per GPU over both transports."""
-import json
 import os
-import socket
-import subprocess
 import sys
 
 import numpy as np
@@ -16,6 +13,7 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from rank_world import run_world  # noqa: E402
 from k1_reference import bf16_to_f32, f32_to_bf16_bits, row_selected, row_terms  # noqa: E402
 from mp_worker import MB_FRACTION, MB_ITERS, make_csr, make_data, minibatch_poisoned  # noqa: E402
 
@@ -32,34 +30,6 @@ def _gpu_count():
         return 0
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn_world(world, devices, transport, out, timeout=420):
-    port = _free_port()
-    env = dict(os.environ, OMP_NUM_THREADS="1")
-    procs = [subprocess.Popen([sys.executable, os.path.join(HERE, "mp_worker.py"), str(r), str(world), str(port),
-                               str(devices[r]), transport, out], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-             for r in range(world)]
-    logs, failed = [], False
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            failed = True
-            for q in procs:          # exactly the PIDs this test started
-                q.kill()
-            o, _ = p.communicate()
-        logs.append(o.decode(errors="replace")[-3000:])
-        failed = failed or p.returncode != 0
-    assert not failed, "a rank failed or hung:\n" + "\n-----\n".join(logs)
-    with open(out) as f:
-        return json.load(f)
-
-
 WORLDS = [("ipc", 2, "same"), ("ipc", 3, "same"), ("ipc", 2, "spread"), ("nccl", 2, "spread")]
 
 
@@ -70,7 +40,7 @@ def test_process_per_rank_world_matches_oracle(oracle, tmp_path, transport, worl
     if placement == "spread" and ngpu < world:
         pytest.skip(f"needs {world} GPUs (the same-device worlds cover the IPC path on this box)")
     devices = list(range(world)) if placement == "spread" else [0] * world
-    res = _spawn_world(world, devices, transport, str(tmp_path / "res.json"))
+    res = run_world("mp_worker.py", world, str(tmp_path / "res.json"), devices=devices, extra=(transport,))
     O = oracle
     # --- applySmooth and the loop on loaded shards, oracle partitions = ranks (the same combOp order, AGD.scala:201-204)
     X, y = make_data(6001, 1024, 7)

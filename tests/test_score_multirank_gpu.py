@@ -1,11 +1,8 @@
 """Scoring in a process-per-rank world (tests/score_worker.py): worlds of 2 and 3 processes share one GPU over the
 host-shipped CUDA IPC exchange.  Margins are rank-local; agd_evaluate reduces over the world and gives every rank the same
 bits; collective calls around an evaluation keep their bits."""
-import json
 import math
 import os
-import socket
-import subprocess
 import sys
 
 import numpy as np
@@ -13,37 +10,11 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from rank_world import run_world  # noqa: E402
 from k1_reference import row_terms  # noqa: E402
 from score_worker import B, N_CSR, N_DENSE, T, csr_data, dense_data, rows_of  # noqa: E402
 
 U = 2.0 ** -53
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(world, out, timeout=420):
-    port = _free_port()
-    env = dict(os.environ, OMP_NUM_THREADS="1")
-    procs = [subprocess.Popen([sys.executable, os.path.join(HERE, "score_worker.py"), str(r), str(world), str(port), "0", out],
-                              env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT) for r in range(world)]
-    logs, failed = [], False
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            failed = True
-            for q in procs:          # exactly the PIDs this test started
-                q.kill()
-            o, _ = p.communicate()
-        logs.append(o.decode(errors="replace")[-3000:])
-        failed = failed or p.returncode != 0
-    assert not failed, "a rank failed or hung:\n" + "\n-----\n".join(logs)
-    with open(out) as f:
-        return json.load(f)
 
 
 def _sums(kind, m, y, t):
@@ -68,7 +39,7 @@ def _check_sums(got, ref):
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 3])
 def test_score_world_over_ipc(tmp_path, world):
-    res = _spawn(world, str(tmp_path / "res.json"))
+    res = run_world("score_worker.py", world, str(tmp_path / "res.json"))
     assert len(res) == world
     X, y, w = dense_data()
     X = X.astype(np.float64)

@@ -1,10 +1,7 @@
 """Views in a process-per-rank world (tests/view_worker.py): worlds of 2 and 3 processes share one GPU over the host-shipped
 CUDA IPC exchange.  A view's smooth, run and evaluate give the same bits on every rank; on a generated shard the view selects
 the rows a 1-rank world selects and the run matches the oracle on them; collective calls after view calls keep their bits."""
-import json
 import os
-import socket
-import subprocess
 import sys
 
 import numpy as np
@@ -12,41 +9,15 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from rank_world import run_world  # noqa: E402
 from view_reference import view_mask  # noqa: E402
 from view_worker import GEN_D, GEN_ROWS, GEN_SEED, SPLIT_SEED  # noqa: E402
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _spawn(world, out, timeout=420):
-    port = _free_port()
-    env = dict(os.environ, OMP_NUM_THREADS="1")
-    procs = [subprocess.Popen([sys.executable, os.path.join(HERE, "view_worker.py"), str(r), str(world), str(port), "0", out],
-                              env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT) for r in range(world)]
-    logs, failed = [], False
-    for p in procs:
-        try:
-            o, _ = p.communicate(timeout=timeout)
-        except subprocess.TimeoutExpired:
-            failed = True
-            for q in procs:          # exactly the PIDs this test started
-                q.kill()
-            o, _ = p.communicate()
-        logs.append(o.decode(errors="replace")[-3000:])
-        failed = failed or p.returncode != 0
-    assert not failed, "a rank failed or hung:\n" + "\n-----\n".join(logs)
-    with open(out) as f:
-        return json.load(f)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 3])
 def test_views_world_over_ipc(tmp_path, oracle, world):
-    res = _spawn(world, str(tmp_path / "res.json"))
+    res = run_world("view_worker.py", world, str(tmp_path / "res.json"))
     assert len(res) == world
     for key in ("loss", "grad", "count", "w", "hist", "eval"):
         assert all(rr["view"][key] == res[0]["view"][key] for rr in res), key
