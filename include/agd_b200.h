@@ -215,6 +215,15 @@ int agd_evaluate(agd_handle *h, int32_t gradient, const double *w, double interc
 enum { AGD_COLSTAT_SUM = 0, AGD_COLSTAT_SUM_SQ, AGD_COLSTAT_SUM_ABS, AGD_COLSTAT_NNZ,
        AGD_COLSTAT_DEV, AGD_COLSTAT_DEV2, AGD_COLSTAT_MAX, AGD_COLSTAT_MIN, AGD_COLSTAT_N };
 int agd_col_stats(agd_handle *h, double *count, double *out);
+/* Cross-products over ALL shards of the world (RowMatrix.computeGramianMatrix / computeCovariance; collective, like
+ * agd_col_stats; agd_set_row_filter applies, agd_set_feature_transform does not).  *count = rows in the view; out =
+ * (agd_dim(h) + 1)^2 doubles, row-major and exactly symmetric: out[i][j] = sum z_i z_j, out[i][d] = out[d][i] = sum z_i,
+ * out[d][d] = count, with z = x (centered = 0) or z = x - mu, mu = fl(sum x / count) (centered = 1; CSR shards derive the
+ * centered sums from the uncentered ones).  Zeros count as values; a row outside the view leaves no trace; sums follow IEEE
+ * arithmetic.  Identical bits on every rank; dense shards also on every repeated call (CSR sums are scattered: equal to
+ * rounding).  agd_dim(h) <= AGD_GRAMIAN_MAX_DIM. */
+enum { AGD_GRAMIAN_MAX_DIM = 8192 };
+int agd_gramian(agd_handle *h, int32_t centered, double *count, double *out);
 /* Ranking metrics over ALL shards of the world (BinaryClassificationMetrics of mllib 1.3.0; collective, like agd_evaluate).
  * Rows: every row of the current view (agd_set_row_filter applies; agd_set_feature_transform does not: score a transformed
  * model with weights s o v and intercept b, as for agd_evaluate); a row outside the view leaves no trace.  A row is positive
@@ -240,7 +249,7 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask), agd_evaluate, agd_col_stats and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate, agd_col_stats, agd_gramian and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */
@@ -257,7 +266,7 @@ int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, 
  * scale: NULL (no scaling) or agd_dim(h) finite doubles; append_bias: 0 or 1.  (NULL, 0) clears the transform.
  * It applies to agd_smooth, agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run and agd_gd_run_minibatch: their weights and
  * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  (agd_prox takes its dimension as an argument.)
- * It does not apply to agd_margins, agd_evaluate, agd_col_stats, the loads or the row accessors, which address the stored
+ * It does not apply to agd_margins, agd_evaluate, agd_col_stats, agd_gramian, the loads or the row accessors, which address the stored
  * features: score a transformed model there with weights s o v and intercept b.
  * The rows are never rewritten: the gradient kernels add b to every margin and sum the multipliers for the intercept's
  * gradient, the point is scaled (w_eff = s o v) before each sweep and the gradient columns after it, so a scaled value is never

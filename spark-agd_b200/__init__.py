@@ -15,6 +15,7 @@ from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Conte
 from .stat import MultivariateStatisticalSummary, Statistics
 from .feature import StandardScaler, StandardScalerModel
 from .evaluation import BinaryClassificationMetrics
+from .linalg import RowMatrix
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -23,4 +24,4 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
            "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics", "StandardScaler",
-           "StandardScalerModel", "physical_model", "BinaryClassificationMetrics"]
+           "StandardScalerModel", "physical_model", "BinaryClassificationMetrics", "RowMatrix"]

@@ -26,6 +26,8 @@ BIN_POS, BIN_NEG, BIN_NAN, BIN_AUROC, BIN_AUPR, BIN_N = range(6)
 # agd_col_stats: rows of the statistic-major block it returns (AGD_COLSTAT_*), COLSTAT_N of them
 (COLSTAT_SUM, COLSTAT_SUM_SQ, COLSTAT_SUM_ABS, COLSTAT_NNZ, COLSTAT_DEV, COLSTAT_DEV2, COLSTAT_MAX, COLSTAT_MIN,
  COLSTAT_N) = range(9)
+# agd_gramian: the largest agd_dim(h) it takes (AGD_GRAMIAN_MAX_DIM; beyond it the call fails and allocates nothing)
+GRAMIAN_MAX_DIM = 8192
 
 
 class Params(C.Structure):
@@ -117,6 +119,7 @@ _SIGNATURES = {
     "agd_margins": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_evaluate": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
     "agd_col_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
+    "agd_gramian": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_void_p]),
     "agd_binary_curve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int64), C.c_void_p]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

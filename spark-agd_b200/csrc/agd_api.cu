@@ -108,6 +108,8 @@ struct Dev {
   double *eval = nullptr;          // AGD_EVAL_N sums of agd_evaluate (this shard's, then the world's)
   double *cs = nullptr;            // agd_col_stats: pass-1 sums, maxima, pass-2 sums, CSR max keys (see colstats_layout)
   size_t cs_doubles = 0;
+  double *gm = nullptr;            // agd_gramian: packed result, mu, pass-1 sums, CSR keys, slabs (see gramian_layout)
+  size_t gm_doubles = 0;
   void *bin[kBinBufs] = {};        // agd_binary_curve scratch (see BinBuf), grown on demand, freed by agd_clear / agd_destroy
   size_t bin_bytes[kBinBufs] = {};
   double *partials = nullptr;
@@ -1088,7 +1090,7 @@ int agd_destroy(agd_handle *h) {
     D.comm = nullptr;
     free_shard(h, D);
     double *v[] = {D.x, D.z, D.x_old, D.z_old, D.y, D.g_y, D.g_x, D.wtmp, D.y_spec, D.acc, D.slabs, D.partials, D.eval, D.cs,
-                   D.tf_scale, D.weff, D.weff2};
+                   D.gm, D.tf_scale, D.weff, D.weff2};
     for (double *p : v)
       if (p) cudaFree(p);
     if (D.ticket) cudaFree(D.ticket);
@@ -1414,6 +1416,9 @@ int agd_clear(agd_handle *h) {
     CK(cudaStreamSynchronize(D.st));
     if (free_shard(h, D)) return 1;
     free_bin(D);
+    if (D.gm) cudaFree(D.gm);
+    D.gm = nullptr;
+    D.gm_doubles = 0;
   }
   h->d = 0;
   h->d_user = 0;
@@ -1762,6 +1767,116 @@ int agd_col_stats(agd_handle *h, double *count, double *out) {
     const double v[AGD_COLSTAT_N] = {sum, r[d + c], r[2 * (size_t)d + c], r[3 * (size_t)d + c], dev, dev2, mx, -nmn};
     for (int k = 0; k < AGD_COLSTAT_N; ++k) out[(size_t)k * du + c] = v[k];
   }
+  return 0;
+}
+
+// ---------------------------------------------------------------- cross-products (gramian.cu)
+// D.gm, in doubles: [packed result P | mu d | pass-1 sums col_sum_n(d) | CSR max keys 2 d | work], P = gramian_packed_n(d); work =
+// the dense sweep's slabs (splits x P), or a CSR shard's uncentered sums (P) when they are centered after
+struct GramianLayout {
+  size_t out, mu, sums, keys, work, total;
+};
+static GramianLayout gramian_layout(int32_t d, size_t work) {
+  GramianLayout L;
+  L.out = 0;
+  L.mu = gramian_packed_n(d);
+  L.sums = L.mu + (size_t)d;
+  L.keys = L.sums + col_sum_n(d);
+  L.work = L.keys + 2 * (size_t)d;
+  L.total = L.work + work;
+  return L;
+}
+
+// Collective.  Centered: colStats pass 1 on every local shard and the exchange of its sums (4 d + 1, the same payload on dense
+// and CSR shards), mu on the device; then the cross-product sweep of every local shard, its packed sums exchanged over the world
+// in epochs of one slot stride.  The host mirrors the packed triangle into the full matrix.
+int agd_gramian(agd_handle *h, int32_t centered, double *count, double *out) {
+  if (check_ready(h)) return 1;
+  if (h->d_user > AGD_GRAMIAN_MAX_DIM)
+    return fail(h, "agd_gramian: d = %d features; the d x d result is limited to d <= %d", h->d_user, AGD_GRAMIAN_MAX_DIM);
+  if (!count || !out) return fail(h, "NULL argument");
+  const int32_t d = h->d, du = h->d_user;
+  const size_t P = gramian_packed_n(d), nsum1 = 4 * (size_t)d + 1;
+  std::vector<int> splits(h->devs.size(), 0);
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    const Shard &s = D.sh;
+    if (!s.csr) splits[i] = gramian_splits(D.sm_count, d, s.rows);
+    const GramianLayout L = gramian_layout(d, s.csr ? (centered ? P : 0) : (size_t)splits[i] * P);
+    if (D.gm_doubles < L.total) {
+      if (D.gm) cudaFree(D.gm);
+      D.gm = nullptr;
+      D.gm_doubles = 0;
+      if (cudaMalloc(&D.gm, L.total * sizeof(double)) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(h, "agd_gramian: cannot allocate %zu bytes of scratch on device %d", L.total * sizeof(double), D.ordinal);
+      }
+      D.gm_doubles = L.total;
+    }
+    if (!centered) continue;
+    ColStatsArgs a;
+    a.rows = s.rows; a.d = d; a.row_base = D.row_base; a.filt = h->filt_of(D); a.stream = D.st;
+    if (s.csr) {
+      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val;
+      a.out = D.gm + L.sums; a.keys = reinterpret_cast<unsigned long long *>(D.gm + L.keys);
+      CK(cudaMemsetAsync(D.gm + L.sums, 0, (col_sum_n(d) + 2 * (size_t)d) * sizeof(double), D.st));
+      CK(colstats_csr_launch(a, 1, s.elem_bytes, D.sm_count));
+    } else {
+      const int mb = colstats_max_blocks(D.sm_count, d);
+      if (ensure_slabs(h, D, mb, (int32_t)(nsum1 + 2 * (size_t)d))) return 1;
+      a.X = s.X; a.slabs = D.slabs; a.max_slabs = D.slabs + (size_t)mb * nsum1;
+      int blocks = 0;
+      CK(colstats_dense_launch(a, 1, s.elem_bytes, D.sm_count, &blocks));
+      CK(k1_reduce_launch(a.slabs, blocks, (int32_t)nsum1, D.gm + L.sums, nullptr, D.st));
+    }
+  }
+  const GramianLayout L = gramian_layout(d, 0);   // every offset below the work area is the same on every device
+  if (centered) {
+    if (world_reduce(h, [&](size_t i) { return h->devs[i].gm + L.sums; }, nsum1, kXchgSum)) return 1;
+    for (Dev &D : h->devs) {
+      CK(cudaSetDevice(D.ordinal));
+      CK(colstats_mu_launch(D.gm + L.sums, d, D.gm + L.mu, D.st));
+    }
+  }
+  for (size_t i = 0; i < h->devs.size(); ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    const Shard &s = D.sh;
+    GramianArgs a;
+    a.rows = s.rows; a.d = d; a.stream = D.st;
+    if (s.csr) {
+      a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; a.row_base = D.row_base; a.filt = h->filt_of(D);
+      a.out = D.gm + (centered ? L.work : L.out);
+      CK(cudaMemsetAsync(a.out, 0, P * sizeof(double), D.st));
+      CK(gramian_csr_launch(a, s.elem_bytes, D.sm_count));
+      if (centered) CK(gramian_center_launch(a.out, D.gm + L.mu, d, D.gm + L.out, D.st));
+    } else {
+      if (ensure_view_bits(h, D)) return 1;
+      a.X = s.X; a.view_bits = h->filt.n ? D.view_bits : nullptr; a.mu = centered ? D.gm + L.mu : nullptr;
+      a.slabs = D.gm + L.work;
+      CK(gramian_dense_launch(a, s.elem_bytes, D.sm_count, splits[i]));
+      CK(k1_reduce_launch(a.slabs, splits[i], (int32_t)P, D.gm + L.out, nullptr, D.st));
+    }
+  }
+  if (world_reduce(h, [&](size_t i) { return h->devs[i].gm + L.out; }, P, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<double> r(P);
+  CK(cudaMemcpyAsync(r.data(), D0.gm + L.out, P * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
+  // internal index k (d = the augmented one) -> the caller's (du); padded columns du .. d - 1 are dropped
+  const size_t n1 = (size_t)du + 1;
+  auto ext = [&](int32_t k) { return k == d ? du : k; };
+  size_t p = 0;
+  for (int32_t i = 0; i <= d; ++i)
+    for (int32_t j = i; j <= d; ++j, ++p) {
+      if ((i >= du && i < d) || (j >= du && j < d)) continue;
+      const size_t a = (size_t)ext(i), b = (size_t)ext(j);
+      out[a * n1 + b] = r[p];
+      out[b * n1 + a] = r[p];
+    }
+  *count = r[P - 1];
   return 0;
 }
 

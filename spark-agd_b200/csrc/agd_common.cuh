@@ -278,6 +278,32 @@ cudaError_t colstats_mu_launch(const double *sums, int32_t d, double *mu, cudaSt
 // out[c] = NaN-ignoring max over the slabs of column c < n, fixed order
 cudaError_t colstats_max_reduce_launch(const double *slabs, int blocks, int32_t n, double *out, cudaStream_t st);
 
+// ---------------------------------------------------------------- cross-products (gramian.cu, agd_gramian)
+// The packed upper triangle of the augmented (d + 1) x (d + 1) matrix [sum z z^T, sum z; sum z^T, count], entry (i, j), i <= j,
+// at i (d + 1) - i (i - 1) / 2 + (j - i): gramian_packed_n(d) doubles.
+struct GramianArgs {
+  const void *X = nullptr;          // dense shard (fp32 / fp64 / bf16), row-major, ld == d
+  const int64_t *rowptr = nullptr;  // CSR shard (fp32 / fp64 values)
+  const int32_t *idx = nullptr;
+  const void *val = nullptr;
+  int64_t rows = 0;
+  int32_t d = 0;
+  long long row_base = 0;           // CSR: global index of the shard's first row ...
+  const RowFilter *filt = nullptr;  // ... and the view (rows outside it are not read)
+  const uint32_t *view_bits = nullptr;   // dense: the view as a bitmap of the shard's rows (nullptr: every row)
+  const double *mu = nullptr;       // dense: d values subtracted from every kept element (nullptr: uncentered)
+  double *slabs = nullptr;          // dense: [splits][gramian_packed_n(d)], every entry written
+  double *out = nullptr;            // CSR: gramian_packed_n(d) doubles (zeroed), scattered with RED.ADD
+  cudaStream_t stream = nullptr;
+};
+size_t gramian_packed_n(int32_t d);
+// row splits of a dense sweep (slabs it writes)
+int gramian_splits(int sm_count, int32_t d, int64_t rows);
+cudaError_t gramian_dense_launch(const GramianArgs &a, int elem_bytes, int sm_count, int splits);
+cudaError_t gramian_csr_launch(const GramianArgs &a, int elem_bytes, int sm_count);
+// out = the centered packed sums derived from the uncentered ones u (the same rows) and the world's mu
+cudaError_t gramian_center_launch(const double *u, const double *mu, int32_t d, double *out, cudaStream_t st);
+
 // out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
 cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);
 // the same predicate as a bitmap: bit i % 32 of bits[i / 32] for rows [0, rows) (ceil(rows / 32) words)

@@ -559,6 +559,19 @@ class DeviceDataset:
                                        _ptr(fp) if n else None, C.byref(k), _ptr(out)), self.h)
         return out, m, tp, fp
 
+    def gramian(self, centered: bool):
+        """The augmented cross-product matrix of the stored features over every shard of the world (agd_gramian; collective:
+        every rank calls it, every rank gets the same bits): (count, A) with A the (d + 1) x (d + 1) matrix [sum z z^T, sum z;
+        sum z^T, count], z = x, or x - mu with mu = fl(sum x / count) when `centered`.  On a transformed view these are the
+        stored features' sums (linalg.augmented_transformed maps them)."""
+        d = self._phys_d
+        out = np.empty((d + 1, d + 1), dtype=np.float64) if d <= N.GRAMIAN_MAX_DIM else np.empty(0)   # larger: the call fails
+        count = C.c_double()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(N.lib().agd_gramian(self.h, 1 if centered else 0, C.byref(count), _ptr(out)), self.h)
+        return count.value, out
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)

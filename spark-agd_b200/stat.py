@@ -101,7 +101,20 @@ class MultivariateStatisticalSummary:
 
 
 class Statistics:
-    """org.apache.spark.mllib.stat.Statistics [mllib-1.3.0] (column summaries)."""
+    """org.apache.spark.mllib.stat.Statistics [mllib-1.3.0] (column summaries and correlations)."""
+
+    @staticmethod
+    def corr(data: DeviceDataset, method: str = "pearson") -> np.ndarray:
+        """The d x d correlation matrix of the columns of a DeviceDataset or view (collective), derived from the covariance
+        as MLlib's computeCorrelationMatrixFromCovariance does: a column with variance <= 1e-12 has NaN correlations and
+        1.0 on the diagonal."""
+        from .linalg import RowMatrix, correlation_from_covariance
+        if method == "spearman":
+            raise NotImplementedError("method='spearman' ranks every column's values over all rows: that needs a per-column "
+                                      "sort of the resident rows, a different kernel; only 'pearson' is implemented")
+        if method != "pearson":
+            raise ValueError(f"unknown correlation method {method!r}: 'pearson' or 'spearman'")
+        return correlation_from_covariance(RowMatrix(data).computeCovariance())
 
     @staticmethod
     def colStats(data: DeviceDataset) -> MultivariateStatisticalSummary:
