@@ -224,6 +224,19 @@ int agd_col_stats(agd_handle *h, double *count, double *out);
  * rounding).  agd_dim(h) <= AGD_GRAMIAN_MAX_DIM. */
 enum { AGD_GRAMIAN_MAX_DIM = 8192 };
 int agd_gramian(agd_handle *h, int32_t centered, double *count, double *out);
+/* RowMatrix.multiply: the rows of h's current view times B (agd_dim(h) x k, row-major, finite fp64) plus offset (k doubles,
+ * NULL = 0), into the EMPTY handle dst opened on the same local device ordinals in the same world position (rank-local, not
+ * collective; agd_set_row_filter of h applies, agd_set_feature_transform does not: fold a transform into B and offset).
+ * On every local device i, dst's shard i then holds the view's rows of h's shard i in physical order, as k features stored as
+ * store_dtype (AGD_F64, AGD_F32 or AGD_BF16), each with its label: exactly the shard a load of those rows would give (the same
+ * padding, kernel and solver).  Every y_ij is an fp64 sum of x_il b_lj over the row's features (a CSR row's stored entries in
+ * stored order, a repeated column adding up) in an order that depends only on agd_dim(h) and k, then + offset_j, rounded
+ * once to nearest-even: the bits of a projected row depend only on that row, B and offset.  Non-finite features follow IEEE
+ * arithmetic; a row outside the view is never read.  Without a row filter dst's rows keep h's numbering (a view of dst selects
+ * the rows the same view of h selects); with one, dst numbers them as a loaded shard.  Fails on a non-empty dst (left as it
+ * is), other devices or world position, k < 1, a non-finite entry of B or offset, or a shard of 2^31 rows or more; a failure
+ * after these checks (e.g. an allocation) leaves dst cleared. */
+int agd_project(agd_handle *h, const double *B, int32_t k, const double *offset, agd_handle *dst, int32_t store_dtype);
 /* Ranking metrics over ALL shards of the world (BinaryClassificationMetrics of mllib 1.3.0; collective, like agd_evaluate).
  * Rows: every row of the current view (agd_set_row_filter applies; agd_set_feature_transform does not: score a transformed
  * model with weights s o v and intercept b, as for agd_evaluate); a row outside the view leaves no trace.  A row is positive
@@ -249,7 +262,7 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask), agd_evaluate, agd_col_stats, agd_gramian and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate, agd_col_stats, agd_gramian, agd_project and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */
@@ -266,7 +279,7 @@ int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, 
  * scale: NULL (no scaling) or agd_dim(h) finite doubles; append_bias: 0 or 1.  (NULL, 0) clears the transform.
  * It applies to agd_smooth, agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run and agd_gd_run_minibatch: their weights and
  * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  (agd_prox takes its dimension as an argument.)
- * It does not apply to agd_margins, agd_evaluate, agd_col_stats, agd_gramian, the loads or the row accessors, which address the stored
+ * It does not apply to agd_margins, agd_evaluate, agd_col_stats, agd_gramian, agd_project, the loads or the row accessors, which address the stored
  * features: score a transformed model there with weights s o v and intercept b.
  * The rows are never rewritten: the gradient kernels add b to every margin and sum the multipliers for the intercept's
  * gradient, the point is scaled (w_eff = s o v) before each sweep and the gradient columns after it, so a scaled value is never

@@ -11,11 +11,12 @@ from .glm import (GeneralizedLinearAlgorithm, GeneralizedLinearModel, LinearRegr
                   LogisticRegressionModel, LogisticRegressionWithAGD, SVMModel, SVMWithAGD, append_bias, column_std)
 from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Context, DeviceDataset, Evaluation, Gradient, GradientDescent,
                            HingeGradient, L1Updater, LeastSquaresGradient, LogisticGradient, MLUtils, RunStats,
-                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, physical_model, run_with_stats, split_bounds)
+                           SimpleUpdater, SquaredL2Updater, Updater, bf16_to_f32, physical_model, physical_projection, run_with_stats,
+                           split_bounds)
 from .stat import MultivariateStatisticalSummary, Statistics
 from .feature import StandardScaler, StandardScalerModel
 from .evaluation import BinaryClassificationMetrics
-from .linalg import RowMatrix
+from .linalg import RowMatrix, SingularValueDecomposition
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -24,4 +25,5 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "HingeGradient", "L1Updater", "LeastSquaresGradient", "LogisticGradient", "MLUtils", "NativeError", "RunStats",
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
            "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics", "StandardScaler",
-           "StandardScalerModel", "physical_model", "BinaryClassificationMetrics", "RowMatrix"]
+           "StandardScalerModel", "physical_model", "physical_projection", "BinaryClassificationMetrics", "RowMatrix",
+           "SingularValueDecomposition"]

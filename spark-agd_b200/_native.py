@@ -120,6 +120,7 @@ _SIGNATURES = {
     "agd_evaluate": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
     "agd_col_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
     "agd_gramian": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.c_void_p]),
+    "agd_project": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32]),
     "agd_binary_curve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int64), C.c_void_p]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1880,6 +1880,100 @@ int agd_gramian(agd_handle *h, int32_t centered, double *count, double *out) {
   return 0;
 }
 
+// ---------------------------------------------------------------- projection (project.cu)
+// Rank-local.  Per local device: the view's bitmap and the exclusive scan of its tile counts (the kept rows, read back), the
+// destination shard reserved as a load of that many rows would reserve it, B and c padded into the source device's staging
+// buffer, and one launch on the source's stream.  Any failure after the checks clears dst.
+static int project_device(agd_handle *h, Dev &D, const std::vector<double> &Bp, const std::vector<double> &cp, int32_t k,
+                          int32_t kp, agd_handle *dst, Dev &E, int32_t store_dtype) {
+  const Shard &s = D.sh;
+  const bool filtered = h->filt.n > 0;
+  const size_t tiles = (size_t)((s.rows + kPjRows - 1) / kPjRows);
+  const size_t bytes = (Bp.size() + cp.size() + tiles + 1) * sizeof(double);
+  CK(cudaSetDevice(D.ordinal));
+  if (D.stage_bytes < bytes) {
+    if (D.stage_dev) cudaFree(D.stage_dev);
+    D.stage_dev = nullptr;
+    D.stage_bytes = 0;
+    if (cudaMalloc(&D.stage_dev, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, "agd_project: cannot allocate %zu bytes of scratch on device %d", bytes, D.ordinal);
+    }
+    D.stage_bytes = bytes;
+  }
+  double *Bd = (double *)D.stage_dev, *cd = Bd + Bp.size();
+  long long *tile_base = (long long *)(cd + cp.size()), *total_d = tile_base + tiles;
+  CK(cudaMemcpyAsync(Bd, Bp.data(), Bp.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  CK(cudaMemcpyAsync(cd, cp.data(), cp.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  long long kept = s.rows;
+  if (filtered && s.rows > 0) {
+    if (ensure_view_bits(h, D)) return 1;
+    CK(project_scan_launch(D.view_bits, s.rows, tile_base, total_d, D.st));
+    CK(cudaMemcpyAsync(&kept, total_d, sizeof kept, cudaMemcpyDeviceToHost, D.st));
+  }
+  CK(cudaStreamSynchronize(D.st));
+  {
+    std::lock_guard<std::mutex> g(*E.mu);
+    if (reserve_locked(dst, E, kept, dst->d, store_dtype)) {
+      const std::string why = dst->err;
+      return fail(h, "agd_project: cannot reserve %zu bytes for %lld rows x %d features on device %d (%s)",
+                  (size_t)kept * dst->d * dtype_bytes(store_dtype) + ((size_t)kept + 64) * sizeof(double), kept, dst->d,
+                  E.ordinal, why.c_str());
+    }
+  }
+  ProjectArgs a;
+  if (s.csr) { a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; }
+  else a.X = s.X;
+  a.labels = s.labels; a.rows = s.rows; a.d = h->d; a.stream = D.st;
+  a.view_bits = filtered ? D.view_bits : nullptr; a.tile_base = filtered ? tile_base : nullptr;
+  a.B = Bd; a.c = cd; a.k = k; a.kp = kp;
+  a.Y = E.sh.X; a.Ylabels = E.sh.labels; a.ldy = dst->d; a.out_bytes = dtype_bytes(store_dtype);
+  if (kept > 0) {
+    if (s.csr) CK(project_csr_launch(a, s.elem_bytes, D.sm_count));
+    else CK(project_dense_launch(a, s.elem_bytes));
+  }
+  CK(cudaStreamSynchronize(D.st));   // dst's own stream never races the rows written on this one
+  E.sh.rows = kept;
+  if (!filtered) E.row_base = D.row_base;   // the same rows, numbered as the source numbers them
+  return 0;
+}
+
+int agd_project(agd_handle *h, const double *B, int32_t k, const double *offset, agd_handle *dst, int32_t store_dtype) {
+  if (!h) return 1;
+  if (!dst || dst == h) return fail(h, "agd_project: dst must be another handle");
+  if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
+  bool empty = dst->d == 0;
+  for (const Dev &E : dst->devs) empty = empty && E.sh.rows == 0 && E.sh.cap == 0;
+  if (!empty) return fail(h, "agd_project: the destination handle is not empty (agd_clear it or open a new one)");
+  bool same = dst->devs.size() == h->devs.size() && dst->world == h->world && dst->first_rank == h->first_rank;
+  for (size_t i = 0; same && i < h->devs.size(); ++i) same = dst->devs[i].ordinal == h->devs[i].ordinal;
+  if (!same) return fail(h, "agd_project: dst must be opened on the same local devices in the same world position as the source");
+  if (k < 1) return fail(h, "agd_project: k = %d columns (at least 1)", k);
+  if (!dtype_bytes(store_dtype)) return fail(h, "store_dtype must be AGD_F64, AGD_F32 or AGD_BF16");
+  if (!B) return fail(h, "NULL argument");
+  const int32_t du = h->d_user;
+  for (size_t q = 0; q < (size_t)du * k; ++q)
+    if (!std::isfinite(B[q])) return fail(h, "agd_project: B[%zu][%zu] = %g is not finite", q / k, q % k, B[q]);
+  if (offset)
+    for (int32_t j = 0; j < k; ++j)
+      if (!std::isfinite(offset[j])) return fail(h, "agd_project: offset[%d] = %g is not finite", j, offset[j]);
+  for (const Dev &D : h->devs)
+    if (D.sh.rows >= (int64_t)1 << 31)
+      return fail(h, "agd_project: %lld rows on device %d (at most 2^31 - 1)", (long long)D.sh.rows, D.ordinal);
+  // B as the kernels read it: [bd][kp], rows padded to whole 16-row chunks and columns to whole column tiles, zeros elsewhere
+  const int32_t bd = (h->d + 15) / 16 * 16, tc = project_tile_cols(k), kp = (k + tc - 1) / tc * tc;
+  std::vector<double> Bp((size_t)bd * kp, 0.0), cp((size_t)kp, 0.0);
+  for (int32_t l = 0; l < du; ++l) memcpy(&Bp[(size_t)l * kp], B + (size_t)l * k, (size_t)k * sizeof(double));
+  if (offset) memcpy(cp.data(), offset, (size_t)k * sizeof(double));
+  if (set_dim(dst, k, dtype_bytes(store_dtype))) return fail(h, "agd_project: %s", dst->err.c_str());
+  for (size_t i = 0; i < h->devs.size(); ++i)
+    if (project_device(h, h->devs[i], Bp, cp, k, kp, dst, dst->devs[i], store_dtype)) {
+      agd_clear(dst);
+      return 1;
+    }
+  return 0;
+}
+
 // ---------------------------------------------------------------- ranking metrics (rank.cu)
 // One shard: the key form of the scoring sweep (rows of the view, non-NaN margins), the radix sort and the run-length reduce
 // into this device's curve (D.bin[kBinList], *len records); *nan = rows of the view whose margin is NaN.

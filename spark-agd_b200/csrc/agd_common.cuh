@@ -304,6 +304,33 @@ cudaError_t gramian_csr_launch(const GramianArgs &a, int elem_bytes, int sm_coun
 // out = the centered packed sums derived from the uncentered ones u (the same rows) and the world's mu
 cudaError_t gramian_center_launch(const double *u, const double *mu, int32_t d, double *out, cudaStream_t st);
 
+// ---------------------------------------------------------------- projection (project.cu, agd_project)
+// Y = X B + c over the rows of a view, compacted in physical order into another handle's dense shard.  B is [bd][kp] doubles,
+// bd = d rounded up to 16 and kp = k rounded up to project_tile_cols(k), zero-padded; c is kp doubles, zero beyond k.
+constexpr int kPjRows = 128;        // rows of X per dense CTA, and the rows per entry of tile_base
+struct ProjectArgs {
+  const void *X = nullptr;          // dense source (fp32 / fp64 / bf16), row-major, ld == d
+  const int64_t *rowptr = nullptr;  // CSR source (fp32 / fp64 values)
+  const int32_t *idx = nullptr;
+  const void *val = nullptr;
+  const double *labels = nullptr;
+  int64_t rows = 0;
+  int32_t d = 0;                    // the source's stored row length
+  const uint32_t *view_bits = nullptr;   // the view as a bitmap of the shard's rows (nullptr: every row) ...
+  const long long *tile_base = nullptr;  // ... and the kept rows before each tile of kPjRows rows (project_scan_launch)
+  const double *B = nullptr;
+  const double *c = nullptr;
+  int32_t k = 0, kp = 0;
+  void *Y = nullptr;                // destination rows, ld == ldy (k, padded as a load pads it), storage out_bytes
+  double *Ylabels = nullptr;
+  int32_t ldy = 0, out_bytes = 8;
+  cudaStream_t stream = nullptr;
+};
+int project_tile_cols(int32_t k);
+cudaError_t project_scan_launch(const uint32_t *bits, int64_t rows, long long *tile_base, long long *total, cudaStream_t st);
+cudaError_t project_dense_launch(const ProjectArgs &a, int elem_bytes);
+cudaError_t project_csr_launch(const ProjectArgs &a, int elem_bytes, int sm_count);
+
 // out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
 cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);
 // the same predicate as a bitmap: bit i % 32 of bits[i / 32] for rows [0, rows) (ceil(rows / 32) words)

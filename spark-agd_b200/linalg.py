@@ -5,12 +5,17 @@ components of a DeviceDataset or view.
   mat.computeGramianMatrix()            # d x d, sum x x^T
   mat.computeCovariance()               # d x d, unbiased
   mat.computePrincipalComponents(k)     # d x k
+  mat.multiply(B)                       # RowMatrix of the rows times B, resident on the same devices
+  mat.computeSVD(k, computeU=True)      # SingularValueDecomposition(U, s, V)
 
 The device returns the augmented cross-products [sum z z^T, sum z; sum z^T, count] over every shard of the world
 (agd_gramian); everything else is derived from that (d + 1) x (d + 1) matrix on the host, in O(d^2) (O(d^3) for the
-eigendecomposition, which MLlib also runs on the driver).
+eigendecomposition, which MLlib also runs on the driver).  multiply projects the rows on the device (agd_project) into a new
+resident dataset.
 """
 from __future__ import annotations
+
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -89,10 +94,39 @@ def principal_components(cov, k: int) -> np.ndarray:
         raise ValueError(f"k = {k} out of range 1 <= k <= n = {d}")
     w, v = np.linalg.eigh(c)
     order = np.argsort(w, kind="stable")[::-1][:k]
-    pc = v[:, order]
-    big = np.argmax(np.abs(pc), axis=0)
-    signs = np.where(pc[big, np.arange(k)] < 0, -1.0, 1.0)
-    return pc * signs[None, :]
+    return _fix_signs(v[:, order])
+
+
+def _fix_signs(m):
+    """Each column times -1 where its entry of largest magnitude (the first of equals) is negative."""
+    big = np.argmax(np.abs(m), axis=0)
+    signs = np.where(m[big, np.arange(m.shape[1])] < 0, -1.0, 1.0)
+    return m * signs[None, :]
+
+
+class SingularValueDecomposition(NamedTuple):
+    """SingularValueDecomposition(U, s, V) of mllib 1.3.0: U a RowMatrix (None unless computeU), s the singular values in
+    descending order, V the d x len(s) right singular vectors."""
+    U: Optional["RowMatrix"]
+    s: np.ndarray
+    V: np.ndarray
+
+
+def svd_from_gramian(G, k: int, rCond: float = 1e-9):
+    """(s, V) of RowMatrix.computeSVD's local path (mllib 1.3.0) from the Gramian G = A^T A: sigma = sqrt of G's singular
+    values, descending; the leading sigma_i >= rCond sigma_0 are kept, at most k of them; V holds the matching singular vectors
+    of G, each column's sign fixed as in principal_components."""
+    g = np.asarray(G, dtype=np.float64)
+    d = g.shape[0]
+    if not (isinstance(k, (int, np.integer)) and 1 <= k <= d):
+        raise ValueError(f"k = {k} out of range 1 <= k <= n = {d}")
+    u, sig2, _ = np.linalg.svd(g)
+    sigma = np.sqrt(sig2)
+    threshold = float(rCond) * sigma[0]
+    sk = 0
+    while sk < k and sigma[sk] >= threshold:
+        sk += 1
+    return sigma[:sk].copy(), _fix_signs(u[:, :sk])
 
 
 class RowMatrix:
@@ -134,6 +168,24 @@ class RowMatrix:
         if not (isinstance(k, (int, np.integer)) and 1 <= k <= d):
             raise ValueError(f"k = {k} out of range 1 <= k <= n = {d}")
         return principal_components(self.computeCovariance(), k)
+
+    def multiply(self, B, store: str = "f64") -> "RowMatrix":
+        """The rows times B ((d, k) array, d = numCols()) as a RowMatrix whose .data is a new resident DeviceDataset (labels
+        kept, stored as `store`), projected on the device without a host copy of the rows (DeviceDataset.project).  A wrong
+        shape, a non-finite entry or k < 1 raises ValueError."""
+        return RowMatrix(self.data.project(B, store=store))
+
+    def computeSVD(self, k: int, computeU: bool = False, rCond: float = 1e-9) -> SingularValueDecomposition:
+        """The top-k singular values and right singular vectors (svd_from_gramian of computeGramianMatrix()), with U =
+        multiply(V diag(1 / s)) when computeU.  MLlib 1.3.0 takes this local path for small or wide requests and ARPACK on the
+        distributed Gramian otherwise; here the Gramian is cheap on the device, so it is always taken and s and V are the exact
+        top k to rounding.  k outside 1 <= k <= numCols() raises ValueError."""
+        d = self.numCols()
+        if not (isinstance(k, (int, np.integer)) and 1 <= k <= d):
+            raise ValueError(f"k = {k} out of range 1 <= k <= n = {d}")
+        s, V = svd_from_gramian(self.computeGramianMatrix(), k, rCond)
+        U = self.multiply(V * (1.0 / s)[None, :]) if computeU else None
+        return SingularValueDecomposition(U, s, V)
 
     def computeColumnSummaryStatistics(self):
         from .stat import Statistics

@@ -572,6 +572,23 @@ class DeviceDataset:
             N.check(N.lib().agd_gramian(self.h, 1 if centered else 0, C.byref(count), _ptr(out)), self.h)
         return count.value, out
 
+    def project(self, B, offset=None, store: str = "f64") -> "DeviceDataset":
+        """RowMatrix.multiply on the device (agd_project): a new dataset whose rows are this dataset's (or view's) rows times B
+        ((d, k) array, d = self.d) plus `offset` (k values, None = 0), stored as `store`, each with its label, in physical
+        order on the same devices.  A transformed view is folded into B and offset first (physical_projection).  Rank-local,
+        but the new dataset is opened on this one's context, so in a multi-process world every rank calls it.  The result owns
+        its shards: close() frees them."""
+        P, c = physical_projection(B, offset, self._scale, self._bias, self.d)
+        out = DeviceDataset(self.ctx)
+        try:
+            with self._filtered():
+                N.check(N.lib().agd_project(self.h, _ptr(P), P.shape[1], _ptr(c), out.h, _STORE[store]), self.h)
+        except BaseException:
+            out.close()
+            raise
+        out.total_rows = sum(out.local_rows(i) for i in range(len(self.ctx.devices)))
+        return out
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
@@ -662,6 +679,30 @@ def physical_model(w, intercept: float, scale=None, bias: bool = False):
     if scale is not None:
         v = v * np.asarray(scale, dtype=np.float64)
     return np.ascontiguousarray(v), float(intercept) + b
+
+
+def physical_projection(B, offset=None, scale=None, bias: bool = False, d: Optional[int] = None):
+    """A projection x -> x B + offset of appendBias(s o x) as one of the stored x: (diag(s) B[:d_stored], offset + B[d_stored])
+    with the bias row folded into the offset when bias (as physical_model folds a model).  B is (d, k) with d the view's
+    width; a wrong shape, k < 1 or a non-finite entry (also one the fold makes) raises ValueError."""
+    B = np.asarray(B, dtype=np.float64)
+    if B.ndim != 2 or B.shape[1] < 1 or (d is not None and B.shape[0] != d):
+        raise ValueError(f"B has shape {B.shape}; it must be (d, k) with d = {d} rows and k >= 1 columns")
+    k = B.shape[1]
+    c = np.zeros(k) if offset is None else np.asarray(offset, dtype=np.float64)
+    if c.shape != (k,):
+        raise ValueError(f"offset has shape {c.shape}; it must be ({k},)")
+    if not (np.all(np.isfinite(B)) and np.all(np.isfinite(c))):
+        raise ValueError("B and offset must be finite")
+    P = B[:-1] if bias else B
+    if bias:
+        c = c + B[-1]
+    if scale is not None:
+        with np.errstate(over="ignore", invalid="ignore"):
+            P = P * np.asarray(scale, dtype=np.float64)[:, None]
+    if not (np.all(np.isfinite(P)) and np.all(np.isfinite(c))):
+        raise ValueError("the projection of the stored features overflows (scale times B is not finite)")
+    return np.ascontiguousarray(P), np.ascontiguousarray(c)
 
 
 def _ratio(a: float, b: float) -> float:
