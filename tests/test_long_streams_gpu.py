@@ -415,9 +415,9 @@ def test_gramian_splits_and_ring(agd, ctx, store, d, rows):
 
 
 # ---------------------------------------------------------------- CSR
-def _csr_design(seed):
+def _csr_design(seed, n=CSR_ROWS):
     rng = np.random.default_rng(seed)
-    n, d, k = CSR_ROWS, CSR_D, 12
+    d, k = CSR_D, 12
     cols = np.sort(rng.integers(0, d, (n, k)), axis=1)
     keep = (np.arange(k) < rng.integers(0, k + 1, n)[:, None])
     keep[:, 1:] &= cols[:, 1:] != cols[:, :-1]                    # one stored entry per column and row
@@ -538,7 +538,8 @@ def test_shard_past_2_31_elements(agd, ctx, store):
     """A 65,536 x 1024 block appended 34 times into a reserved shard: 2.28e9 elements (4.6 GB in bf16, 9.1 GB in fp32).
     Every reference follows from the block: sums are 34 x the block's, the margins are the block's tiled, the curve's counts
     are 34 x the block's at the same keys.  The least-squares gradient is exact too: every fp32 margin, every bf16 x 3 split
-    of a residual and every 16-row fp32 sum of the wgmma kernel is an integer below 2^24."""
+    of a residual and every 16-row fp32 sum of the wgmma kernel is an integer below 2^24.  So is the projection, whose rows
+    are the block's projected rows tiled (tests/test_project_long_gpu.py's exact design)."""
     rows_b, d, reps = 65536, 1024, 34
     dz = Design(d, rows_b // 2, 1, 0, seed=31)
     n = rows_b * reps
@@ -577,5 +578,21 @@ def test_shard_past_2_31_elements(agd, ctx, store):
             loss, g, c = ds.smooth(agd.LeastSquaresGradient(), dz.w)
             assert c == n and loss == L / n, (variant, loss, L / n)
             assert np.array_equal(bits(g), bits(S / n)), (variant, np.flatnonzero(g != S / n)[:5])
+        # the projection, with B and c in 2^-20 Z (exact: every sum is below 2^14): the block's rows tiled, into fp64 at k = 16,
+        # into fp32 at k = 130 (two column tiles), and through a sample view of 17,408 row tiles (17 per scan thread).  Each
+        # projection is closed before the next.
+        from test_project_long_gpu import check_rows, exact_B, exact_projection, expected_bits
+        rng = np.random.default_rng(32)
+        ridx = np.arange(n) % rows_b
+        view = ds.sample(False, 0.37, seed=5)
+        for src, dest, k, sel in ((ds, "f64", 16, ridx), (ds, "f32", 130, ridx),
+                                  (view, "f64", 16, ridx[view.row_mask(0, 0, n)])):
+            Bp, cp = exact_B(rng, d, k)
+            want = expected_bits(exact_projection(xb, Bp, cp), dest)
+            p = src.project(Bp, cp, store=dest)
+            try:
+                check_rows(p, dest, k, want, sel, yb)
+            finally:
+                p.close()
     finally:
         ds.close()
