@@ -255,6 +255,43 @@ enum { AGD_BIN_POS = 0, AGD_BIN_NEG, AGD_BIN_NAN, AGD_BIN_AUROC, AGD_BIN_AUPR, A
 int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t capacity, double *margin_out, int64_t *tp_out,
                      int64_t *fp_out, int64_t *n_points, double *out);
 
+/* ---- clustering the resident shards (KMeans of mllib 1.3.0) ----
+ * Every call works on the rows of the current view in its feature space: agd_set_row_filter applies (a row outside the view is
+ * never read, so a non-finite feature in one leaves no trace) and so does agd_set_feature_transform, so a row is
+ * z = appendBias(s o x), D = agd_dim(h) + append_bias features, s o x formed in fp64.  Centres are k x D finite doubles,
+ * row-major; sums and sampled rows have D entries per row.
+ * A row's centre is the lowest index j minimising the score ||c_j||^2 - 2 z . c_j, with z . c_j the fp64 sum agd_project forms
+ * (x . (s o c_j), plus the bias entry of c_j; dense shards: DMMA in an order that depends only on agd_dim(h) and k; CSR: the
+ * stored entries in stored order).  A NaN score never wins; a row no centre wins goes to centre 0.  The centre therefore
+ * depends only on the row and the centres, and differs from the exact argmin only where the two best exact distances lie
+ * within the cross term's rounding.  Distances and costs are exact residuals sum_l (z_l - c_l)^2 in fp64 (a CSR row:
+ * ||c||^2 + the sum over its stored entries, and the bias, of (z_l - c_l)^2 - c_l^2).  Shards of 2^31 rows or more are refused.
+ * Scratch (about 40 bytes per local row, 12 more per 128 centres beyond the first 128, and 8 for agd_kmeans_costs' per-row
+ * cost) stays on the handle until agd_clear / agd_destroy. */
+/* One Lloyd step over ALL shards of the world (collective): every row of the view assigned to its centre; sums_out (k x D, NULL =
+ * not returned) = the sum of each centre's rows, counts_out (k) = their number, *cost_out = the sum of every row's residual to
+ * its centre.  One exchange of k (D + 1) + 1 doubles.  Dense sums are fp64 in a fixed order (the rows sorted stably by centre,
+ * pieces of 4096 rows added in order): identical bits on every rank and every repeated call.  CSR sums and cost are scattered
+ * with fp64 RED.ADD: equal to rounding.  Counts are exact. */
+int agd_kmeans_step(agd_handle *h, const double *centers, int32_t k, double *sums_out, double *counts_out, double *cost_out);
+/* Centres of physical rows [row0, row0 + rows) of the shard on local device dev (rank-local, not collective, like agd_margins):
+ * cluster_out[i] = the row's centre, or -1 for a row outside the view; dist_out (NULL = not returned) = its residual (NaN
+ * outside the view). */
+int agd_kmeans_assign(agd_handle *h, int32_t dev, const double *centers, int32_t k, int64_t row0, int64_t rows,
+                      int32_t *cluster_out, double *dist_out);
+/* The cost update of k-means|| (collective): every row of the view gets delta = its residual to the centre among these m
+ * candidates that it is assigned to, or with keep the smaller of that and its previous delta (a NaN residual never replaces
+ * it); *sum_out = the sum of delta over the world, added in a fixed order (identical bits on every rank and repeated call).
+ * delta stays on the handle (8 bytes per local row) for agd_kmeans_sample.  keep needs a previous call on the same rows. */
+int agd_kmeans_costs(agd_handle *h, const double *centers, int32_t m, int32_t keep, double *sum_out);
+/* The rows of the view kept by the k-means draw (collective): row r is kept iff u < factor * delta_r (weighted = 1, delta of
+ * the last agd_kmeans_costs) or u < factor (weighted = 0), u = the top 53 bits of the row's Philox draw u(seed, grow) of
+ * stream 8 (see agd_set_row_filter) as a double in [0, 1).  *n_out = rows kept over the world; when capacity >= *n_out,
+ * rows_out (n x D) holds them as fp64 features of the view's space and draws_out (NULL = not returned) their u, in rank order
+ * and physical order within a rank.  capacity 0 asks for the count only.  factor must be finite and >= 0. */
+int agd_kmeans_sample(agd_handle *h, uint64_t seed, double factor, int32_t weighted, int64_t capacity, double *rows_out,
+                      double *draws_out, int64_t *n_out);
+
 /* ---- views of the resident shards (RDD.randomSplit / sample / MLUtils.kFold without copying a row) ----
  * Every row has a 64-bit draw u = Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, 7), words 0 and 1, where grow
  * = the shard's first global row + local row (the numbering of the mini-batch mask: a generated shard's global row, or
@@ -262,7 +299,8 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask), agd_evaluate, agd_col_stats, agd_gramian, agd_project and agd_binary_curve, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate, agd_col_stats, agd_gramian, agd_project, agd_binary_curve, agd_kmeans_step, agd_kmeans_assign, agd_kmeans_costs
+ * and agd_kmeans_sample, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */
@@ -278,7 +316,8 @@ int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, 
  * appended as the last feature (MLUtils.appendBias): the intercept is the last weight, regularised like every other.
  * scale: NULL (no scaling) or agd_dim(h) finite doubles; append_bias: 0 or 1.  (NULL, 0) clears the transform.
  * It applies to agd_smooth, agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run and agd_gd_run_minibatch: their weights and
- * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  (agd_prox takes its dimension as an argument.)
+ * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  It applies to agd_kmeans_step, agd_kmeans_assign,
+ * agd_kmeans_costs and agd_kmeans_sample too: their centres, sums and rows have agd_dim(h) + append_bias entries.  (agd_prox takes its dimension as an argument.)
  * It does not apply to agd_margins, agd_evaluate, agd_col_stats, agd_gramian, agd_project, the loads or the row accessors, which address the stored
  * features: score a transformed model there with weights s o v and intercept b.
  * The rows are never rewritten: the gradient kernels add b to every margin and sum the multipliers for the intercept's

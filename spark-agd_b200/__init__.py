@@ -17,6 +17,7 @@ from .stat import MultivariateStatisticalSummary, Statistics
 from .feature import StandardScaler, StandardScalerModel
 from .evaluation import BinaryClassificationMetrics
 from .linalg import RowMatrix, SingularValueDecomposition
+from .clustering import KMeans, KMeansModel, LocalKMeans
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -26,4 +27,4 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
            "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics", "StandardScaler",
            "StandardScalerModel", "physical_model", "physical_projection", "BinaryClassificationMetrics", "RowMatrix",
-           "SingularValueDecomposition"]
+           "SingularValueDecomposition", "KMeans", "KMeansModel", "LocalKMeans"]

@@ -123,6 +123,11 @@ _SIGNATURES = {
     "agd_project": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32]),
     "agd_binary_curve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int64), C.c_void_p]),
+    "agd_kmeans_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]),
+    "agd_kmeans_assign": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "agd_kmeans_costs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),
+    "agd_kmeans_sample": (C.c_int, [C.c_void_p, C.c_uint64, C.c_double, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                    C.POINTER(C.c_int64)]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "agd_row_filter_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_set_feature_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

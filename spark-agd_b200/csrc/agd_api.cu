@@ -91,6 +91,22 @@ enum BinBuf {
   kBinCurve,              // the world's curve
   kBinBufs
 };
+// agd_kmeans_* scratch buffers on a device
+enum KmBuf {
+  kKmCluster,             // each row's centre (int32), or each sampled row's bit
+  kKmDelta,               // agd_kmeans_costs' per-row cost
+  kKmCentres,             // the centres as the kernels read them: B | cb | cn | C
+  kKmTiles,               // per column tile: best score (double) of each row | its index (int32)
+  kKmKeys0, kKmKeys1,     // the stable sort of (centre, row)
+  kKmVals0, kKmVals1,
+  kKmSortTiles,           // the sort's per-tile digit counts
+  kKmMisc,                // [8 x 256 digit counts | counts (k + 1) u64] / sampling: [tile_base | total] | lengths
+  kKmPieces,              // pstart | pcl | pfirst of the dense sums
+  kKmPart,                // per-piece sums | per-piece residuals | column residuals
+  kKmPayload,             // [sums k x md | counts k | cost], exchanged over the world
+  kKmRows,                // sampled rows, this device's at its rank's block of the world's
+  kKmBufs
+};
 constexpr size_t kBinMiscCounters = 8 * 256 * sizeof(unsigned), kBinMiscRuns = kBinMiscCounters + 8,
                  kBinMiscAreas = kBinMiscRuns + 8, kBinMiscOwn = kBinMiscAreas + 16, kBinMiscAll = kBinMiscOwn + 16;
 
@@ -112,6 +128,9 @@ struct Dev {
   size_t gm_doubles = 0;
   void *bin[kBinBufs] = {};        // agd_binary_curve scratch (see BinBuf), grown on demand, freed by agd_clear / agd_destroy
   size_t bin_bytes[kBinBufs] = {};
+  void *km[kKmBufs] = {};          // agd_kmeans_* scratch (see KmBuf), grown on demand, freed by agd_clear / agd_destroy
+  size_t km_bytes[kKmBufs] = {};
+  int64_t km_delta_rows = -1;      // rows kKmDelta describes (-1: no agd_kmeans_costs since the last load or clear)
   double *partials = nullptr;
   unsigned int *ticket = nullptr;
   double *scalars_dev = nullptr;   // device alias of scalars_host: K3 writes its scalars straight to the host
@@ -176,6 +195,7 @@ struct agd_handle {
   // in which the intercept is the last weight (index d internally, d_user for the caller).
   bool tf_scale = false;
   int32_t tf_bias = 0;
+  std::vector<double> tf_scale_host;   // the scale factors, d_user of them (k-means folds them into its centres on the host)
   int32_t model_d() const { return d + tf_bias; }
   const double *scale_of(const Dev &D) const { return tf_scale ? D.tf_scale : nullptr; }
   int collective = 0;        // 0 = auto (peer memory if every pair of ranks can map each other, else NCCL), 1 = nccl, 2 = p2p
@@ -379,6 +399,28 @@ void free_bin(Dev &D) {
     D.bin[i] = nullptr;
     D.bin_bytes[i] = 0;
   }
+}
+void free_km(Dev &D) {
+  for (int i = 0; i < kKmBufs; ++i) {
+    if (D.km[i]) cudaFree(D.km[i]);
+    D.km[i] = nullptr;
+    D.km_bytes[i] = 0;
+  }
+  D.km_delta_rows = -1;
+}
+
+int ensure_km(agd_handle *h, Dev &D, int which, size_t bytes) {
+  if (D.km_bytes[which] >= bytes) return 0;
+  if (D.km[which]) cudaFree(D.km[which]);
+  D.km[which] = nullptr;
+  D.km_bytes[which] = 0;
+  if (which == kKmDelta) D.km_delta_rows = -1;
+  if (cudaMalloc(&D.km[which], bytes) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(h, "agd_kmeans: cannot allocate %zu bytes of scratch on device %d", bytes, D.ordinal);
+  }
+  D.km_bytes[which] = bytes;
+  return 0;
 }
 
 // The current filter as a bitmap of D's rows, drawn by the kernels' own row_in_view() (one launch, one Philox per row and
@@ -1100,6 +1142,7 @@ int agd_destroy(agd_handle *h) {
     if (D.filt_dev) cudaFree(D.filt_dev);
     if (D.view_bits) cudaFree(D.view_bits);
     free_bin(D);
+    free_km(D);
     for (cudaEvent_t e : D.ev) cudaEventDestroy(e);
     for (cudaEvent_t e : D.ev_ar) cudaEventDestroy(e);
     if (&D == &h->devs[0] && h->ev_begin) { cudaEventDestroy(h->ev_begin); cudaEventDestroy(h->ev_end); }
@@ -1416,6 +1459,7 @@ int agd_clear(agd_handle *h) {
     CK(cudaStreamSynchronize(D.st));
     if (free_shard(h, D)) return 1;
     free_bin(D);
+    free_km(D);
     if (D.gm) cudaFree(D.gm);
     D.gm = nullptr;
     D.gm_doubles = 0;
@@ -2138,6 +2182,321 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
   return 0;
 }
 
+// ---------------------------------------------------------------- clustering (kmeans.cu)
+// The centres as the kernels read them, built once on the host for every device: C [k][md] in the internal width md = d + bias
+// (zeros on padded columns), B [round_up(d, 16)][kp] = (s o C)^T zero-padded, cb = the bias entries, cn = ||c_j||^2 added over
+// the columns in order.
+struct KmCentres {
+  int32_t k = 0, kp = 0, md = 0;
+  std::vector<double> buf;   // B | cb | cn | C
+  size_t nB = 0;
+};
+static int km_centres(agd_handle *h, const char *what, const double *centers, int32_t k, KmCentres &c) {
+  if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
+  if (k < 1) return fail(h, "%s: k = %d centres (at least 1)", what, k);
+  if (!centers) return fail(h, "NULL argument");
+  for (const Dev &D : h->devs)
+    if (D.sh.rows >= (int64_t)1 << 31) return fail(h, "%s: %lld rows on device %d (at most 2^31 - 1)", what, (long long)D.sh.rows, D.ordinal);
+  const int32_t du = h->d_user, d = h->d, b = h->tf_bias, Dx = du + b;
+  for (size_t q = 0; q < (size_t)k * Dx; ++q)
+    if (!std::isfinite(centers[q])) return fail(h, "%s: centre %zu, feature %zu = %g is not finite", what, q / Dx, q % Dx, centers[q]);
+  const int32_t tc = project_tile_cols(k), bd = (d + 15) / 16 * 16;
+  c.k = k; c.kp = (k + tc - 1) / tc * tc; c.md = d + b;
+  c.nB = (size_t)bd * c.kp;
+  c.buf.assign(c.nB + 2 * (size_t)c.kp + (size_t)k * c.md, 0.0);
+  double *B = c.buf.data(), *cb = B + c.nB, *cn = cb + c.kp, *C = cn + c.kp;
+  for (int32_t j = 0; j < k; ++j) {
+    const double *src = centers + (size_t)j * Dx;
+    double *cj = C + (size_t)j * c.md;
+    for (int32_t l = 0; l < du; ++l) {
+      cj[l] = src[l];
+      B[(size_t)l * c.kp + j] = h->tf_scale ? h->tf_scale_host[(size_t)l] * src[l] : src[l];
+    }
+    if (b) cb[j] = cj[d] = src[du];
+    double n = 0.0;
+    for (int32_t l = 0; l < c.md; ++l) n += cj[l] * cj[l];
+    cn[j] = n;
+  }
+  return 0;
+}
+
+// D's arguments for the rows [0, rows) of its shard, the centres uploaded
+static int km_args(agd_handle *h, Dev &D, const KmCentres &c, KmeansArgs &a) {
+  const Shard &s = D.sh;
+  CK(cudaSetDevice(D.ordinal));
+  if (ensure_km(h, D, kKmCentres, c.buf.size() * sizeof(double))) return 1;
+  double *dev = (double *)D.km[kKmCentres];
+  CK(cudaMemcpyAsync(dev, c.buf.data(), c.buf.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  if (h->filt.n && ensure_view_bits(h, D)) return 1;
+  a = KmeansArgs();
+  if (s.csr) { a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; }
+  else a.X = s.X;
+  a.rows = s.rows; a.d = h->d; a.md = c.md; a.bias = h->tf_bias; a.scale = h->scale_of(D);
+  a.view_bits = h->filt.n ? D.view_bits : nullptr;
+  a.k = c.k; a.kp = c.kp;
+  a.B = dev; a.cb = dev + c.nB; a.cn = a.cb + c.kp; a.C = a.cn + c.kp;
+  a.stream = D.st;
+  return 0;
+}
+
+// centres of rows [a.row0, a.row0 + a.rows) into D.km[kKmCluster]
+static int km_assign(agd_handle *h, Dev &D, KmeansArgs &a) {
+  const size_t r1 = a.rows > 0 ? (size_t)a.rows : 1;
+  if (ensure_km(h, D, kKmCluster, r1 * sizeof(int32_t))) return 1;
+  a.cluster = (int32_t *)D.km[kKmCluster];
+  if (!a.rowptr && a.kp > 128) {
+    const size_t tiles = (size_t)a.kp / 128;
+    if (ensure_km(h, D, kKmTiles, tiles * r1 * (sizeof(double) + sizeof(int32_t)))) return 1;
+    a.tile_score = (double *)D.km[kKmTiles];
+    a.tile_idx = (int32_t *)(a.tile_score + tiles * r1);
+  }
+  CK(kmeans_assign_launch(a, D.sh.elem_bytes, D.sm_count));
+  return 0;
+}
+
+// One device's share of a step: the payload [sums k x md | counts k | cost] in D.km[kKmPayload]
+static int km_step_device(agd_handle *h, Dev &D, const KmCentres &c) {
+  KmeansArgs a;
+  if (km_args(h, D, c, a) || km_assign(h, D, a)) return 1;
+  const Shard &s = D.sh;
+  const int32_t k = c.k, md = c.md;
+  const size_t P = (size_t)k * md + k + 1, r1 = s.rows > 0 ? (size_t)s.rows : 1;
+  if (ensure_km(h, D, kKmPayload, P * sizeof(double)) || ensure_km(h, D, kKmMisc, 8 * 256 * sizeof(unsigned) + ((size_t)k + 1) * 8) ||
+      ensure_km(h, D, kKmKeys0, 8 * r1) || ensure_km(h, D, kKmVals0, 4 * r1))
+    return 1;
+  double *pay = (double *)D.km[kKmPayload];
+  unsigned *hist = (unsigned *)D.km[kKmMisc];
+  unsigned long long *counts = (unsigned long long *)(hist + 8 * 256);
+  unsigned long long *keys[2] = {(unsigned long long *)D.km[kKmKeys0], nullptr};
+  void *vals[2] = {D.km[kKmVals0], nullptr};
+  CK(cudaMemsetAsync(pay, 0, P * sizeof(double), D.st));
+  CK(cudaMemsetAsync(counts, 0, ((size_t)k + 1) * 8, D.st));
+  CK(kmeans_keys_launch(a.cluster, s.rows, k, keys[0], (uint32_t *)vals[0], counts, D.st));
+  if (s.csr) {
+    CK(kmeans_sums_csr_launch(a, s.elem_bytes, D.sm_count, pay));
+  } else if (s.rows > 0) {
+    // rows sorted stably by centre, then each centre's rows in pieces of kKmPiece, every piece's columns added in sorted order
+    if (ensure_km(h, D, kKmKeys1, 8 * r1) || ensure_km(h, D, kKmVals1, 4 * r1) ||
+        ensure_km(h, D, kKmSortTiles, bin_sort_tile_words(s.rows) * sizeof(unsigned)))
+      return 1;
+    keys[1] = (unsigned long long *)D.km[kKmKeys1];
+    vals[1] = D.km[kKmVals1];
+    int which = 0, passes = 0;
+    CK(bin_sort_pairs(keys, vals, 4, s.rows, hist, (unsigned *)D.km[kKmSortTiles], &which, &passes, D.st));   // synchronises
+    std::vector<unsigned long long> cnt((size_t)k);
+    CK(cudaMemcpyAsync(cnt.data(), counts, (size_t)k * 8, cudaMemcpyDeviceToHost, D.st));
+    CK(cudaStreamSynchronize(D.st));
+    std::vector<long long> pstart;
+    std::vector<int32_t> pcl, pfirst((size_t)k + 1);
+    long long off = 0;
+    for (int32_t j = 0; j < k; ++j) {
+      pfirst[(size_t)j] = (int32_t)pcl.size();
+      for (long long q = 0; q < (long long)cnt[(size_t)j]; q += kKmPiece) {
+        pstart.push_back(off + q);
+        pcl.push_back(j);
+      }
+      off += (long long)cnt[(size_t)j];
+    }
+    pfirst[(size_t)k] = (int32_t)pcl.size();
+    pstart.push_back(off);
+    const long long np = (long long)pcl.size();
+    const size_t pbytes = pstart.size() * 8 + (pcl.size() + pfirst.size()) * 4;
+    if (ensure_km(h, D, kKmPieces, pbytes) || ensure_km(h, D, kKmPart, (2 * (size_t)np + 1) * md * sizeof(double))) return 1;
+    long long *ps = (long long *)D.km[kKmPieces];
+    int32_t *pc = (int32_t *)(ps + pstart.size()), *pf = pc + pcl.size();
+    CK(cudaMemcpyAsync(ps, pstart.data(), pstart.size() * 8, cudaMemcpyHostToDevice, D.st));
+    if (np) CK(cudaMemcpyAsync(pc, pcl.data(), pcl.size() * 4, cudaMemcpyHostToDevice, D.st));
+    CK(cudaMemcpyAsync(pf, pfirst.data(), pfirst.size() * 4, cudaMemcpyHostToDevice, D.st));
+    double *part = (double *)D.km[kKmPart], *pres = part + (size_t)np * md, *colres = pres + (size_t)np * md;
+    CK(kmeans_sums_dense_launch(a, s.elem_bytes, (const uint32_t *)vals[which], ps, pc, np, part, pres));
+    CK(kmeans_sums_reduce_launch(part, pres, pf, np, k, md, pay, colres, D.st));
+    CK(cudaStreamSynchronize(D.st));   // pstart / pcl / pfirst live on this stack frame until the copies ran
+  }
+  CK(kmeans_counts_launch(counts, k, md, pay, D.st));
+  return 0;
+}
+
+int agd_kmeans_step(agd_handle *h, const double *centers, int32_t k, double *sums_out, double *counts_out, double *cost_out) {
+  KmCentres c;
+  if (check_ready(h) || km_centres(h, "agd_kmeans_step", centers, k, c)) return 1;
+  if (!counts_out || !cost_out) return fail(h, "NULL argument");
+  for (Dev &D : h->devs)
+    if (km_step_device(h, D, c)) return 1;
+  const size_t P = (size_t)k * c.md + k + 1;
+  if (world_reduce(h, [&](size_t i) { return (double *)h->devs[i].km[kKmPayload]; }, P, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<double> r(P);
+  CK(cudaMemcpyAsync(r.data(), D0.km[kKmPayload], P * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
+  const int32_t du = h->d_user, Dx = du + h->tf_bias;
+  for (int32_t j = 0; j < k; ++j) {
+    if (sums_out) model_values(h, &r[(size_t)j * c.md], 1.0, sums_out + (size_t)j * Dx);
+    counts_out[j] = r[(size_t)k * c.md + j];
+  }
+  *cost_out = r[P - 1];
+  return 0;
+}
+
+int agd_kmeans_assign(agd_handle *h, int32_t dev, const double *centers, int32_t k, int64_t row0, int64_t rows,
+                      int32_t *cluster_out, double *dist_out) {
+  if (!h) return 1;
+  if (dev < 0 || dev >= (int)h->devs.size()) return fail(h, "bad local device index %d", dev);
+  KmCentres c;
+  if (km_centres(h, "agd_kmeans_assign", centers, k, c)) return 1;
+  Dev &D = h->devs[dev];
+  if (row0 < 0 || rows < 0 || rows > D.sh.rows - row0)
+    return fail(h, "row range [%lld, %lld + %lld) lies outside the %lld rows of device %d", (long long)row0, (long long)row0,
+                (long long)rows, (long long)D.sh.rows, dev);
+  if (rows > 0 && !cluster_out) return fail(h, "NULL argument");
+  if (rows == 0) return 0;
+  KmeansArgs a;
+  if (km_args(h, D, c, a)) return 1;
+  // a row's centre depends on the row only, so the range is assigned in chunks through the staging buffer
+  const int64_t chunk = rows < (int64_t)(1 << 22) ? rows : (int64_t)(1 << 22);
+  if (dist_out && ensure_stage(h, D, (size_t)chunk * sizeof(double))) return 1;
+  for (int64_t r0 = 0; r0 < rows; r0 += chunk) {
+    a.row0 = row0 + r0;
+    a.rows = rows - r0 < chunk ? rows - r0 : chunk;
+    if (km_assign(h, D, a)) return 1;
+    CK(cudaMemcpyAsync(cluster_out + r0, a.cluster, (size_t)a.rows * sizeof(int32_t), cudaMemcpyDeviceToHost, D.st));
+    if (dist_out) {
+      int blocks = 0;
+      CK(kmeans_dist_launch(a, D.sh.elem_bytes, D.sm_count, (double *)D.stage_dev, nullptr, 0, nullptr, &blocks));
+      CK(cudaMemcpyAsync(dist_out + r0, D.stage_dev, (size_t)a.rows * sizeof(double), cudaMemcpyDeviceToHost, D.st));
+    }
+    CK(cudaStreamSynchronize(D.st));   // the buffers are reused
+  }
+  return 0;
+}
+
+int agd_kmeans_costs(agd_handle *h, const double *centers, int32_t m, int32_t keep, double *sum_out) {
+  KmCentres c;
+  if (check_ready(h) || km_centres(h, "agd_kmeans_costs", centers, m, c)) return 1;
+  if (!sum_out) return fail(h, "NULL argument");
+  if (keep != 0 && keep != 1) return fail(h, "agd_kmeans_costs: keep must be 0 or 1 (got %d)", keep);
+  if (keep)
+    for (const Dev &D : h->devs)
+      if (D.km_delta_rows != D.sh.rows)
+        return fail(h, "agd_kmeans_costs: keep = 1 needs a previous agd_kmeans_costs on the same rows of device %d", D.ordinal);
+  for (Dev &D : h->devs) {
+    KmeansArgs a;
+    if (km_args(h, D, c, a) || km_assign(h, D, a)) return 1;
+    const size_t r1 = D.sh.rows > 0 ? (size_t)D.sh.rows : 1;
+    if (D.km_bytes[kKmDelta] < r1 * sizeof(double) && ensure_km(h, D, kKmDelta, r1 * sizeof(double))) return 1;
+    if (ensure_km(h, D, kKmPayload, sizeof(double))) return 1;
+    const int mb = kmeans_dist_blocks(D.sm_count);
+    if (ensure_slabs(h, D, mb, 1)) return 1;
+    int blocks = 0;
+    CK(kmeans_dist_launch(a, D.sh.elem_bytes, D.sm_count, nullptr, (double *)D.km[kKmDelta], keep, D.slabs, &blocks));
+    CK(k1_reduce_launch(D.slabs, blocks, 1, (double *)D.km[kKmPayload], nullptr, D.st));
+    D.km_delta_rows = D.sh.rows;
+  }
+  if (world_reduce(h, [&](size_t i) { return (double *)h->devs[i].km[kKmPayload]; }, 1, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  CK(cudaMemcpyAsync(sum_out, D0.km[kKmPayload], sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
+  return 0;
+}
+
+int agd_kmeans_sample(agd_handle *h, uint64_t seed, double factor, int32_t weighted, int64_t capacity, double *rows_out,
+                      double *draws_out, int64_t *n_out) {
+  if (check_ready(h)) return 1;
+  if (!n_out) return fail(h, "NULL argument");
+  if (!(factor >= 0.0) || !std::isfinite(factor)) return fail(h, "agd_kmeans_sample: factor must be finite and >= 0 (got %g)", factor);
+  if (weighted != 0 && weighted != 1) return fail(h, "agd_kmeans_sample: weighted must be 0 or 1 (got %d)", weighted);
+  if (capacity < 0) return fail(h, "capacity must be >= 0 (got %lld)", (long long)capacity);
+  if (capacity > 0 && !rows_out) return fail(h, "NULL argument");
+  for (const Dev &D : h->devs) {
+    if (D.sh.rows >= (int64_t)1 << 31)
+      return fail(h, "agd_kmeans_sample: %lld rows on device %d (at most 2^31 - 1)", (long long)D.sh.rows, D.ordinal);
+    if (weighted && D.km_delta_rows != D.sh.rows)
+      return fail(h, "agd_kmeans_sample: weighted = 1 needs a previous agd_kmeans_costs on the same rows of device %d", D.ordinal);
+  }
+  const int W = h->world, nd = (int)h->devs.size();
+  const int32_t md = h->d + h->tf_bias, du = h->d_user, Dx = du + h->tf_bias;
+  const size_t ld1 = (size_t)md + 1;   // a sampled row and its draw
+  std::vector<long long> len((size_t)nd);
+  std::vector<KmeansArgs> args((size_t)nd);
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    const Shard &s = D.sh;
+    CK(cudaSetDevice(D.ordinal));
+    if (h->filt.n && ensure_view_bits(h, D)) return 1;
+    const size_t words = (size_t)((s.rows + 31) / 32) + 1, tiles = (size_t)((s.rows + kPjRows - 1) / kPjRows);
+    if (ensure_km(h, D, kKmCluster, words * 4) || ensure_km(h, D, kKmMisc, (tiles + 2) * 8 + 16 * ((size_t)W + 1))) return 1;
+    KmeansArgs &a = args[(size_t)i];
+    if (s.csr) { a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; }
+    else a.X = s.X;
+    a.rows = s.rows; a.d = h->d; a.md = md; a.bias = h->tf_bias; a.scale = h->scale_of(D);
+    a.view_bits = h->filt.n ? D.view_bits : nullptr; a.stream = D.st;
+    uint32_t *bits = (uint32_t *)D.km[kKmCluster];
+    long long *tile_base = (long long *)D.km[kKmMisc], *total = tile_base + tiles;
+    long long n = 0;
+    if (s.rows > 0) {
+      CK(kmeans_sample_bits_launch(a, seed, D.row_base, factor, weighted ? (const double *)D.km[kKmDelta] : nullptr, bits));
+      CK(project_scan_launch(bits, s.rows, tile_base, total, D.st));
+      CK(cudaMemcpyAsync(&n, total, sizeof n, cudaMemcpyDeviceToHost, D.st));
+      CK(cudaStreamSynchronize(D.st));
+    }
+    len[(size_t)i] = n;
+  }
+  // every rank's count, then every rank's rows at rank r's block of lmax rows
+  std::vector<long long> all(len);
+  if (W > 1) {
+    auto lens = [&](size_t i) {
+      const Dev &D = h->devs[i];
+      const size_t tiles = (size_t)((D.sh.rows + kPjRows - 1) / kPjRows);
+      return (double *)D.km[kKmMisc] + tiles + 2;
+    };
+    for (int i = 0; i < nd; ++i) {
+      Dev &D = h->devs[i];
+      CK(cudaSetDevice(D.ordinal));
+      const double v = (double)len[(size_t)i];
+      CK(cudaMemcpyAsync(lens(i), &v, sizeof v, cudaMemcpyHostToDevice, D.st));
+      CK(cudaStreamSynchronize(D.st));   // v is on this stack frame
+    }
+    if (world_concat(h, lens, 1, [&](size_t i) { return lens(i) + 1; })) return 1;
+    std::vector<double> got((size_t)W);
+    Dev &D0 = h->devs[0];
+    CK(cudaSetDevice(D0.ordinal));
+    CK(cudaMemcpyAsync(got.data(), lens(0) + 1, (size_t)W * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+    if (sync_all(h)) return 1;
+    all.assign((size_t)W, 0);
+    for (int r = 0; r < W; ++r) all[(size_t)r] = (long long)got[(size_t)r];
+  }
+  long long total = 0, lmax = 0;
+  for (long long n : all) { total += n; lmax = std::max(lmax, n); }
+  *n_out = total;
+  if (total == 0 || capacity < total) return 0;
+  const size_t blk = (size_t)lmax * ld1;
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    CK(cudaSetDevice(D.ordinal));
+    if (ensure_km(h, D, kKmRows, (W > 1 ? (size_t)W : 1) * (blk > 0 ? blk : 1) * sizeof(double))) return 1;
+    double *out = (double *)D.km[kKmRows] + (W > 1 ? (size_t)(h->first_rank + i) * blk : 0);
+    if (len[(size_t)i] > 0)
+      CK(kmeans_sample_rows_launch(args[(size_t)i], D.sh.elem_bytes, seed, D.row_base, (const uint32_t *)D.km[kKmCluster],
+                                   (const long long *)D.km[kKmMisc], out, D.sm_count));
+  }
+  auto rows_of = [h](size_t i) { return (double *)h->devs[i].km[kKmRows]; };
+  if (W > 1 && world_concat(h, [&](size_t i) { return rows_of(i) + (size_t)(h->first_rank + (int)i) * blk; }, blk, rows_of)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<double> host((W > 1 ? (size_t)W : 1) * blk);
+  CK(cudaMemcpyAsync(host.data(), D0.km[kKmRows], host.size() * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
+  size_t o = 0;
+  for (size_t r = 0; r < all.size(); ++r)
+    for (long long q = 0; q < all[r]; ++q, ++o) {
+      const double *z = host.data() + r * blk + (size_t)q * ld1;
+      model_values(h, z, 1.0, rows_out + o * Dx);
+      if (draws_out) draws_out[o] = z[md];
+    }
+  return 0;
+}
+
 // ---------------------------------------------------------------- views (row filters)
 int agd_set_row_filter(agd_handle *h, int32_t n, const uint64_t *seeds, const double *lo, const double *hi,
                        const int32_t *complement) {
@@ -2226,6 +2585,7 @@ int agd_set_feature_transform(agd_handle *h, const double *scale, int32_t append
     if (scale) CK(cudaMemcpyAsync(D.tf_scale, s.data(), s.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
     CK(cudaStreamSynchronize(D.st));
   }
+  h->tf_scale_host.assign(s.begin(), s.begin() + h->d_user);
   h->tf_scale = scale != nullptr;
   h->tf_bias = append_bias;
   return 0;

@@ -331,6 +331,64 @@ cudaError_t project_scan_launch(const uint32_t *bits, int64_t rows, long long *t
 cudaError_t project_dense_launch(const ProjectArgs &a, int elem_bytes);
 cudaError_t project_csr_launch(const ProjectArgs &a, int elem_bytes, int sm_count);
 
+// ---------------------------------------------------------------- k-means (kmeans.cu, agd_kmeans_*)
+// Rows [row0, row0 + rows) of one shard in the feature space z = appendBias(s o x) of md = d + bias columns, against k centres.
+// A row's centre is the lowest index j minimising the score ||c_j||^2 - 2 (x . B_j + cb_j) with B_lj = s_l c_jl: the cross term
+// is the projection's fp64 sum (pj_tile.cuh, or a CSR row's stored entries in stored order); a NaN score never wins.
+constexpr int kKmPiece = 4096;      // sorted rows per piece of the dense sums
+struct KmeansArgs {
+  const void *X = nullptr;          // dense shard (fp32 / fp64 / bf16), row-major, ld == d
+  const int64_t *rowptr = nullptr;  // CSR shard (fp32 / fp64 values)
+  const int32_t *idx = nullptr;
+  const void *val = nullptr;
+  long long row0 = 0, rows = 0;
+  int32_t d = 0;                    // stored row length
+  int32_t md = 0;                   // d + bias: columns of C
+  int32_t bias = 0;                 // 1: z_d = 1.0
+  const double *scale = nullptr;    // d factors s (nullptr: s = 1)
+  const uint32_t *view_bits = nullptr;   // the view as a bitmap of the shard's rows (nullptr: every row)
+  int32_t k = 0, kp = 0;            // centres, and k rounded up to whole column tiles (project_tile_cols)
+  const double *B = nullptr;        // [round_up(d, 16)][kp], zero-padded
+  const double *cb = nullptr;       // kp: each centre's bias entry (0 without one)
+  const double *cn = nullptr;       // kp: ||c_j||^2
+  const double *C = nullptr;        // [k][md]: the centres
+  int32_t *cluster = nullptr;       // rows: the row's centre, -1 outside the view
+  double *tile_score = nullptr;     // [kp / 128][rows] and ...
+  int32_t *tile_idx = nullptr;      // ... the best of each 128-column tile, when kp > 128
+  cudaStream_t stream = nullptr;
+};
+cudaError_t kmeans_assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count);
+// Exact residual sum_l (z_l - c_l)^2 of each row of the range to its cluster's centre (CSR: ||c||^2 + sum over the stored
+// entries of (z_l - c_l)^2 - c_l^2, the bias column counted as stored).  dist != nullptr: dist[i] (NaN outside the view).
+// Else delta[i] = the residual, or with keep the smaller of it and delta[i] (a NaN residual never replaces delta[i]), and the
+// view's sum of delta per block into slabs (*blocks_out of them, added in order by k1_reduce_launch).
+int kmeans_dist_blocks(int sm_count);
+cudaError_t kmeans_dist_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *dist, double *delta, int keep,
+                               double *slabs, int *blocks_out);
+// keys[i] = cluster[i] (k outside the view), vals[i] = i, counts[keys[i]] += 1 (counts: k + 1 zeroed words)
+cudaError_t kmeans_keys_launch(const int32_t *cluster, long long rows, int32_t k, unsigned long long *keys, uint32_t *vals,
+                               unsigned long long *counts, cudaStream_t st);
+// Dense sums over pieces of the rows sorted by cluster: piece p is sorted positions [pstart[p], pstart[p + 1]) of cluster
+// pcl[p]; part[p][c] = sum z_c, pres[p][c] = sum (z_c - C[pcl[p]][c])^2, each a sequential fp64 sum in sorted order.
+cudaError_t kmeans_sums_dense_launch(const KmeansArgs &a, int elem_bytes, const uint32_t *order, const long long *pstart,
+                                     const int32_t *pcl, long long npieces, double *part, double *pres);
+// out[j][c] = the pieces pfirst[j] .. pfirst[j + 1] - 1 of part added in order; out[k md + k] = the cost, pres added over the
+// pieces in order per column, then over the columns in order
+cudaError_t kmeans_sums_reduce_launch(const double *part, const double *pres, const int32_t *pfirst, long long npieces,
+                                      int32_t k, int32_t md, double *out, double *colres, cudaStream_t st);
+// CSR: out[j][c] += z_c and out[k md + k] += the row's residual, by fp64 RED.ADD (out zeroed by the caller)
+cudaError_t kmeans_sums_csr_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *out);
+// out[k md + j] = counts[j], j < k
+cudaError_t kmeans_counts_launch(const unsigned long long *counts, int32_t k, int32_t md, double *out, cudaStream_t st);
+// k-means sampling: row r of the view is kept iff u < factor delta[r] (delta = 1 when delta == nullptr), u = the row's draw of
+// stream kKmStream under seed as a double in [0, 1) (the top 53 bits); bit r % 32 of bits[r / 32]
+constexpr uint32_t kKmStream = 8;
+cudaError_t kmeans_sample_bits_launch(const KmeansArgs &a, unsigned long long seed, long long row_base, double factor,
+                                      const double *delta, uint32_t *bits);
+// the kept rows, compacted through tile_base (project_scan_launch of bits): out[o] = [z (md doubles) | u]
+cudaError_t kmeans_sample_rows_launch(const KmeansArgs &a, int elem_bytes, unsigned long long seed, long long row_base,
+                                      const uint32_t *bits, const long long *tile_base, double *out, int sm_count);
+
 // out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
 cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);
 // the same predicate as a bitmap: bit i % 32 of bits[i / 32] for rows [0, rows) (ceil(rows / 32) words)

@@ -15,38 +15,15 @@
 #include <stdint.h>
 
 #include "agd_common.cuh"
-#include "dmma.cuh"
+#include "pj_tile.cuh"
 
 namespace agd {
 
 namespace {
 
-constexpr int kPjThreads = 256;         // 8 warps
-constexpr int kPjKc = 16;               // columns of X (rows of B) per stage
-constexpr int kPjStages = 4;            // ring depth: two chunks in flight while one is multiplied and the next widened
-constexpr int kPjLda = kPjKc + 4;       // fp64 tile row stride: the fragment reads of a half-warp hit 16 distinct 8-byte banks
 constexpr int kPjScanThreads = 1024;
 constexpr int kPjCsrThreads = 256;
 constexpr int kPjCsrCols = 4;           // output columns per lane and pass of the CSR kernel
-constexpr long long kPjMaxGridY = 65535;
-
-// Warp layout of a BN-column tile: WM x WN warps, each owning MT 16-row by NT 8-column MMA tiles.  LDB = BN + 4 keeps the B
-// fragment reads of a half-warp on distinct banks.
-template <int BN> struct PjShape {
-  static constexpr int WN = BN >= 32 ? BN / 32 : 1;
-  static constexpr int WM = 8 / WN;
-  static constexpr int MT = kPjRows / (16 * WM);
-  static constexpr int NT = BN / (8 * WN);
-  static constexpr int LDB = BN + 4;
-};
-
-// Smem (dynamic): B ring [kPjStages][kPjKc][LDB] fp64 | X ring [kPjStages][kPjRows][kPjKc] storage elements | fp64 tiles
-// [2][kPjRows][kPjLda] | output row of each tile row [kPjRows]
-template <typename T, int BN>
-__host__ __device__ constexpr size_t pj_smem_bytes() {
-  return (size_t)kPjStages * kPjKc * PjShape<BN>::LDB * sizeof(double) + (size_t)kPjStages * kPjRows * kPjKc * sizeof(T) +
-         2 * (size_t)kPjRows * kPjLda * sizeof(double) + (size_t)kPjRows * sizeof(long long);
-}
 
 __device__ __forceinline__ void pj_store(void *Y, int out_bytes, long long at, double y) {
   if (out_bytes == 8) reinterpret_cast<double *>(Y)[at] = y;
@@ -54,16 +31,10 @@ __device__ __forceinline__ void pj_store(void *Y, int out_bytes, long long at, d
   else reinterpret_cast<__nv_bfloat16 *>(Y)[at] = __double2bfloat16(y);
 }
 
-// Destination row of physical row `row` (-1: outside the view): its rank among the kept rows, from the kept rows before its
-// tile (tile_base) and the bitmap words of the tile up to it.
+// Destination row of physical row `row` (-1: outside the view)
 __device__ __forceinline__ long long pj_out_row(const ProjectArgs &a, long long row) {
   if (!a.view_bits) return row;
-  const uint32_t w = a.view_bits[row >> 5];
-  if (!((w >> (row & 31)) & 1u)) return -1;
-  const long long t = row / kPjRows;
-  long long o = a.tile_base[t];
-  for (long long q = t * (kPjRows / 32); q < (row >> 5); ++q) o += __popc(a.view_bits[q]);
-  return o + __popc(w & ((1u << (row & 31)) - 1u));
+  return view_rank(a.view_bits, a.tile_base, row);
 }
 
 // tile_base[t] = kept rows in tiles 0 .. t - 1, *total = kept rows of the shard (one CTA; each thread a contiguous run of tiles)
@@ -99,105 +70,19 @@ __global__ void __launch_bounds__(kPjScanThreads) project_scan_kernel(const uint
 }
 
 // VEC: rows are whole 16-byte vectors (d * sizeof(T) % 16 == 0), staged with cp.async; else plain loads.  Row tile rt0 +
-// blockIdx.y, column tile blockIdx.x (the column tiles of one row tile run side by side and share its rows through L2).
+// blockIdx.y, column tile blockIdx.x.
 template <typename T, bool VEC, int BN>
 __global__ void __launch_bounds__(kPjThreads, BN == 128 ? 1 : 2) project_dense_kernel(const ProjectArgs a, const long long rt0) {
   using S = PjShape<BN>;
   extern __shared__ __align__(16) unsigned char pj_smem[];
-  double *bring = reinterpret_cast<double *>(pj_smem);
-  T *xring = reinterpret_cast<T *>(bring + (size_t)kPjStages * kPjKc * S::LDB);
-  double *at = reinterpret_cast<double *>(xring + (size_t)kPjStages * kPjRows * kPjKc);
-  long long *orow = reinterpret_cast<long long *>(at + 2 * kPjRows * kPjLda);
-
-  const int d = a.d, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  long long *orow = pj_orow<T, BN>(pj_smem);
+  const int tid = threadIdx.x;
   const long long r0 = (rt0 + blockIdx.y) * kPjRows;
   const int c0 = (int)blockIdx.x * BN;
-  const T *X = reinterpret_cast<const T *>(a.X);
   if (tid < kPjRows) orow[tid] = r0 + tid < a.rows ? pj_out_row(a, r0 + tid) : -1;
   __syncthreads();
-
-  const int nch = (d + kPjKc - 1) / kPjKc;
-  // stage kc % kPjStages <- columns [kc kPjKc, + kPjKc) of the tile's rows and the same rows of B's column tile; a row outside the
-  // view or past the shard, and columns past d, are not read (zeros)
-  auto issue = [&](int kc) {
-    if (kc >= nch) return;
-    const int s = kc % kPjStages, col0 = kc * kPjKc;
-    double *bs = bring + (size_t)s * kPjKc * S::LDB;
-    for (int u = tid; u < kPjKc * (BN / 2); u += kPjThreads) {
-      const int r = u / (BN / 2), cu = u % (BN / 2);
-      gm_cp16((uint32_t)__cvta_generic_to_shared(bs + r * S::LDB + cu * 2), a.B + (size_t)(col0 + r) * a.kp + c0 + cu * 2, 16);
-    }
-    T *xs = xring + (size_t)s * kPjRows * kPjKc;
-    if (VEC) {
-      constexpr int EPV = 16 / sizeof(T), UPR = kPjKc / EPV;   // 16-byte units per row of a chunk
-      for (int u = tid; u < kPjRows * UPR; u += kPjThreads) {
-        const int r = u / UPR, col = col0 + (u % UPR) * EPV;
-        const bool ok = orow[r] >= 0 && col < d;
-        const T *src = ok ? X + (size_t)(r0 + r) * d + col : X;
-        gm_cp16((uint32_t)__cvta_generic_to_shared(xs + r * kPjKc + (u % UPR) * EPV), src, ok ? 16 : 0);
-      }
-    } else {
-      for (int e = tid; e < kPjRows * kPjKc; e += kPjThreads) {
-        const int r = e / kPjKc, col = col0 + e % kPjKc;
-        T v;
-        if (orow[r] >= 0 && col < d) v = X[(size_t)(r0 + r) * d + col];
-        else memset(&v, 0, sizeof v);
-        xs[e] = v;
-      }
-    }
-  };
-  // chunk kc of the X ring -> fp64 tile zb, every element widened once
-  auto convert = [&](int kc, int zb) {
-    const T *xs = xring + (size_t)(kc % kPjStages) * kPjRows * kPjKc;
-    double *z = at + (size_t)zb * kPjRows * kPjLda;
-#pragma unroll
-    for (int e = tid; e < kPjRows * kPjKc; e += kPjThreads) z[(e / kPjKc) * kPjLda + e % kPjKc] = GmElem<T>::wide(xs[e]);
-  };
-
   double acc[S::MT][S::NT][4];
-#pragma unroll
-  for (int i = 0; i < S::MT; ++i)
-#pragma unroll
-    for (int j = 0; j < S::NT; ++j)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.0;
-  const int wm = warp / S::WN, wn = warp % S::WN;
-
-  for (int q = 0; q < kPjStages - 1; ++q) {
-    issue(q);
-    gm_commit();
-  }
-  if (nch > 0) {
-    gm_wait<kPjStages - 2>();
-    __syncthreads();
-    convert(0, 0);
-  }
-  for (int kc = 0; kc < nch; ++kc) {
-    gm_wait<kPjStages - 3>();
-    __syncthreads();   // chunk kc + 1 landed and chunk kc is widened, for every thread; the MMAs of chunk kc - 1 are done
-    issue(kc + kPjStages - 1);   // into the stage of chunk kc - 1
-    gm_commit();
-    const double *As = at + (size_t)(kc & 1) * kPjRows * kPjLda;
-    const double *Bs = bring + (size_t)(kc % kPjStages) * kPjKc * S::LDB;
-#pragma unroll
-    for (int ks = 0; ks < kPjKc / 4; ++ks) {
-      const int kr = ks * 4 + (lane & 3);
-      double af[S::MT][2], bf[S::NT];
-#pragma unroll
-      for (int mt = 0; mt < S::MT; ++mt) {
-        const int m = wm * S::MT * 16 + mt * 16 + (lane >> 2);
-        af[mt][0] = As[m * kPjLda + kr];
-        af[mt][1] = As[(m + 8) * kPjLda + kr];
-      }
-#pragma unroll
-      for (int nt = 0; nt < S::NT; ++nt) bf[nt] = Bs[kr * S::LDB + wn * S::NT * 8 + nt * 8 + (lane >> 2)];
-#pragma unroll
-      for (int mt = 0; mt < S::MT; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < S::NT; ++nt) gm_dmma(acc[mt][nt], af[mt], bf[nt]);
-    }
-    if (kc + 1 < nch) convert(kc + 1, (kc + 1) & 1);
-  }
+  pj_tile_mma<T, VEC, BN>(pj_smem, reinterpret_cast<const T *>(a.X), a.d, a.B, a.kp, r0, c0, acc);
 
   // y = acc + c_j, rounded once; the destination's padded columns k .. ldy - 1 are written as 0
 #pragma unroll
@@ -206,8 +91,8 @@ __global__ void __launch_bounds__(kPjThreads, BN == 128 ? 1 : 2) project_dense_k
     for (int nt = 0; nt < S::NT; ++nt)
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const int i = wm * S::MT * 16 + mt * 16 + (lane >> 2) + (q >> 1) * 8;
-        const int j = c0 + wn * S::NT * 8 + nt * 8 + (lane & 3) * 2 + (q & 1);
+        const int i = pj_frag_row<BN>(mt, q);
+        const int j = c0 + pj_frag_col<BN>(nt, q);
         const long long o = orow[i];
         if (o >= 0 && j < a.ldy) pj_store(a.Y, a.out_bytes, o * a.ldy + j, j < a.k ? acc[mt][nt][q] + a.c[j] : 0.0);
       }
@@ -247,22 +132,9 @@ __global__ void __launch_bounds__(kPjCsrThreads) project_csr_kernel(const Projec
   }
 }
 
-template <int BN> constexpr bool pj_bn_ok = BN == 16 || BN == 32 || BN == 64 || BN == 128;
-
 template <typename T, bool VEC, int BN>
 cudaError_t launch_dense(const ProjectArgs &a) {
-  static_assert(pj_bn_ok<BN>, "column tile");
-  auto kern = project_dense_kernel<T, VEC, BN>;
-  constexpr size_t smem = pj_smem_bytes<T, BN>();
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  const long long tiles = (a.rows + kPjRows - 1) / kPjRows;
-  for (long long rt0 = 0; rt0 < tiles; rt0 += kPjMaxGridY) {
-    const long long n = tiles - rt0 < kPjMaxGridY ? tiles - rt0 : kPjMaxGridY;
-    kern<<<dim3((unsigned)(a.kp / BN), (unsigned)n), kPjThreads, smem, a.stream>>>(a, rt0);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  }
-  return cudaSuccess;
+  return pj_launch_rows<T, BN>(project_dense_kernel<T, VEC, BN>, a, a.rows, a.kp / BN, a.stream);
 }
 
 template <typename T, int BN>

@@ -589,6 +589,74 @@ class DeviceDataset:
         out.total_rows = sum(out.local_rows(i) for i in range(len(self.ctx.devices)))
         return out
 
+    # clustering (agd_kmeans_*): in this dataset's (or view's) feature space, d = self.d columns, transform applied on the device
+    def _centers(self, centers) -> np.ndarray:
+        c = np.ascontiguousarray(centers, dtype=np.float64)
+        if c.ndim != 2 or c.shape[0] < 1 or c.shape[1] != self.d:
+            raise ValueError(f"centres have shape {c.shape}, data has {self.d} features")
+        return c
+
+    def kmeans_step(self, centers, sums: bool = True):
+        """One Lloyd step over every shard of the world (agd_kmeans_step; collective: every rank gets the same bits):
+        (sums, counts, cost) -- each centre's sum of its rows ((k, d), None unless `sums`) and their count, and the sum of every
+        row's squared distance to its centre."""
+        c = self._centers(centers)
+        k = c.shape[0]
+        s = np.empty((k, self.d), dtype=np.float64) if sums else None
+        counts = np.empty(k, dtype=np.float64)
+        cost = C.c_double()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(N.lib().agd_kmeans_step(self.h, _ptr(c), k, _ptr(s), _ptr(counts), C.byref(cost)), self.h)
+        return s, counts, cost.value
+
+    def kmeans_costs(self, centers, keep: bool) -> float:
+        """The k-means|| cost update (agd_kmeans_costs; collective): each row's cost becomes its squared distance to its
+        closest of `centers`, or the smaller of that and its previous cost with `keep`; returns their sum over the world."""
+        c = self._centers(centers)
+        out = C.c_double()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(N.lib().agd_kmeans_costs(self.h, _ptr(c), c.shape[0], 1 if keep else 0, C.byref(out)), self.h)
+        return out.value
+
+    def kmeans_sample(self, seed: int, factor: float, weighted: bool):
+        """The rows kept by the k-means draw (agd_kmeans_sample; collective): u < factor * cost (weighted, the costs of the
+        last kmeans_costs) or u < factor, with u the row's own draw under `seed`.  (rows (n, d), draws (n,)) in rank order."""
+        L = N.lib()
+        n = C.c_int64()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(L.agd_kmeans_sample(self.h, int(seed) & (2 ** 64 - 1), float(factor), 1 if weighted else 0, 0, None, None,
+                                        C.byref(n)), self.h)
+            rows, draws = np.empty((n.value, self.d), dtype=np.float64), np.empty(n.value, dtype=np.float64)
+            if n.value:
+                N.check(L.agd_kmeans_sample(self.h, int(seed) & (2 ** 64 - 1), float(factor), 1 if weighted else 0, n.value,
+                                            _ptr(rows), _ptr(draws), C.byref(n)), self.h)
+        return rows, draws
+
+    def kmeans_assign_rows(self, dev: int, row0: int, rows: int, centers):
+        """Closest centre (-1 outside the view) and squared distance (NaN outside it) of physical rows [row0, row0 + rows) of
+        local device `dev`'s shard (agd_kmeans_assign; not collective)."""
+        c = self._centers(centers)
+        cl = np.empty(max(int(rows), 0), dtype=np.int32)
+        dist = np.empty(max(int(rows), 0), dtype=np.float64)
+        with self._filtered():
+            N.check(N.lib().agd_kmeans_assign(self.h, dev, _ptr(c), c.shape[0], int(row0), int(rows), _ptr(cl), _ptr(dist)),
+                    self.h)
+        return cl, dist
+
+    def kmeans_assign(self, centers):
+        """(cluster, distance) of this process's rows, across its local devices in load order (not collective); on a view, of
+        the view's rows only, in the same order as margins."""
+        cls, dists = [], []
+        for i in range(len(self.ctx.devices)):
+            cl, dist = self.kmeans_assign_rows(i, 0, self.local_rows(i), centers)
+            keep = cl >= 0
+            cls.append(cl[keep])
+            dists.append(dist[keep])
+        return np.concatenate(cls), np.concatenate(dists)
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
