@@ -292,6 +292,36 @@ int agd_kmeans_costs(agd_handle *h, const double *centers, int32_t m, int32_t ke
 int agd_kmeans_sample(agd_handle *h, uint64_t seed, double factor, int32_t weighted, int64_t capacity, double *rows_out,
                       double *draws_out, int64_t *n_out);
 
+/* ---- classifying the resident shards (NaiveBayes and MulticlassMetrics of mllib 1.3.0) ----
+ * Labels are compared by value (-0.0 is 0.0).  Like the clustering calls, these work on the rows of the current view
+ * (agd_set_row_filter applies; a row outside the view is never read) in its feature space (agd_set_feature_transform applies:
+ * z = appendBias(s o x), D = agd_dim(h) + append_bias features).  Class labels passed in ascend strictly and are not NaN, at
+ * most AGD_MAX_CLASSES of them.  Shards of 2^31 rows or more are refused.  Scratch stays on the handle until agd_clear /
+ * agd_destroy.  The JNI shim does not bind these calls. */
+enum { AGD_MAX_CLASSES = 1024 };
+/* The distinct labels of the view over ALL shards of the world (collective; the distinct values of MLlib's labels), ascending,
+ * with exact counts; *nan_out = rows of the view whose label is NaN (not among the labels).  *n_out = distinct labels; they and
+ * counts_out are written only when capacity >= *n_out (capacity 0 asks for the counts only, as agd_binary_curve does).  The
+ * sort and reduce are agd_binary_curve's, over a key that orders labels ascending. */
+int agd_label_classes(agd_handle *h, int64_t capacity, double *labels_out, int64_t *counts_out, int64_t *n_out,
+                      int64_t *nan_out);
+/* Per class over ALL shards of the world (collective; the aggregate of NaiveBayes.run): the rows of the view whose label equals
+ * labels[c] give counts_out[c] = their number and sums_out[c] (C x D, row-major) = the sum of their features; *negative_out =
+ * the entries of those rows that are not >= 0 (NaN included; a CSR row's stored entries only).  One exchange of C (D + 1) + 1
+ * doubles.  The sums are agd_kmeans_step's: dense shards add each class's rows in a fixed order (identical bits on every rank
+ * and repeated call), CSR shards scatter with fp64 RED.ADD (equal to rounding).  Counts are exact. */
+int agd_class_sums(agd_handle *h, const double *labels, int32_t C, double *sums_out, double *counts_out, double *negative_out);
+/* The linear model's class of physical rows [row0, row0 + rows) of the shard on local device dev (rank-local, not collective,
+ * like agd_kmeans_assign; NaiveBayesModel.predict): class_out[i] = the lowest c maximising offset_c + z . W_c, or -1 for a row
+ * outside the view.  W is C x D finite doubles, row-major, offset C finite doubles; z . W_c is the fp64 sum agd_kmeans_assign
+ * forms.  A NaN score never wins; a row no class wins goes to class 0. */
+int agd_linear_argmax(agd_handle *h, int32_t dev, const double *W, int32_t C, const double *offset, int64_t row0, int64_t rows,
+                      int32_t *class_out);
+/* counts_out (L x C doubles, row-major) = the rows of the view over ALL shards of the world (collective) whose label equals
+ * labels[l] and whose agd_linear_argmax class is c; exact.  C is at most AGD_MAX_CLASSES too. */
+int agd_linear_confusion(agd_handle *h, const double *W, int32_t C, const double *offset, const double *labels, int32_t L,
+                         double *counts_out);
+
 /* ---- views of the resident shards (RDD.randomSplit / sample / MLUtils.kFold without copying a row) ----
  * Every row has a 64-bit draw u = Philox4x32-10 keyed by `seed`, counter (grow lo, grow hi, 0, 7), words 0 and 1, where grow
  * = the shard's first global row + local row (the numbering of the mini-batch mask: a generated shard's global row, or
@@ -299,8 +329,8 @@ int agd_kmeans_sample(agd_handle *h, uint64_t seed, double factor, int32_t weigh
  * floor(lo[i] 2^64) <= u < floor(hi[i] 2^64), with hi = 1 meaning "to the end"; complement[i] = 1 negates it.  A row is in
  * the view iff all n predicates hold (n <= 4).  agd_set_row_filter installs the view; it applies to agd_smooth,
  * agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run, agd_gd_run_minibatch (a row must then also pass the mini-batch
- * mask), agd_evaluate, agd_col_stats, agd_gramian, agd_project, agd_binary_curve, agd_kmeans_step, agd_kmeans_assign, agd_kmeans_costs
- * and agd_kmeans_sample, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
+ * mask), agd_evaluate, agd_col_stats, agd_gramian, agd_project, agd_binary_curve, agd_kmeans_step, agd_kmeans_assign, agd_kmeans_costs,
+ * agd_kmeans_sample, agd_label_classes, agd_class_sums, agd_linear_argmax and agd_linear_confusion, and not to agd_margins, agd_get_rows or the loads, which address physical rows.  Rows outside the
  * view are never touched: a non-finite feature in one leaves no trace.  The filter stays until it is replaced, cleared
  * (n = 0) or dropped by agd_clear; every rank must set the same filter before a collective call.  Bounds must satisfy
  * 0 <= lo <= hi <= 1 and complement must be 0 or 1.  A view still streams the whole shard through the gradient kernels. */
@@ -317,7 +347,8 @@ int agd_row_filter_mask(agd_handle *h, int32_t dev, int64_t row0, int64_t rows, 
  * scale: NULL (no scaling) or agd_dim(h) finite doubles; append_bias: 0 or 1.  (NULL, 0) clears the transform.
  * It applies to agd_smooth, agd_smooth_pair, agd_smooth_two, agd_run, agd_gd_run and agd_gd_run_minibatch: their weights and
  * gradients then have agd_dim(h) + append_bias doubles, the intercept last.  It applies to agd_kmeans_step, agd_kmeans_assign,
- * agd_kmeans_costs and agd_kmeans_sample too: their centres, sums and rows have agd_dim(h) + append_bias entries.  (agd_prox takes its dimension as an argument.)
+ * agd_kmeans_costs and agd_kmeans_sample too: their centres, sums and rows have agd_dim(h) + append_bias entries; and to
+ * agd_class_sums, agd_linear_argmax and agd_linear_confusion: their sums and W rows have agd_dim(h) + append_bias entries.  (agd_prox takes its dimension as an argument.)
  * It does not apply to agd_margins, agd_evaluate, agd_col_stats, agd_gramian, agd_project, the loads or the row accessors, which address the stored
  * features: score a transformed model there with weights s o v and intercept b.
  * The rows are never rewritten: the gradient kernels add b to every margin and sum the multipliers for the intercept's

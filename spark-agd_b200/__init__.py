@@ -15,9 +15,10 @@ from .optimization import (DEFAULT_SPLIT_SEED, AcceleratedGradientDescent, Conte
                            split_bounds)
 from .stat import MultivariateStatisticalSummary, Statistics
 from .feature import StandardScaler, StandardScalerModel
-from .evaluation import BinaryClassificationMetrics
+from .evaluation import BinaryClassificationMetrics, MulticlassMetrics
 from .linalg import RowMatrix, SingularValueDecomposition
 from .clustering import KMeans, KMeansModel, LocalKMeans
+from .classification import NaiveBayes, NaiveBayesModel
 
 __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegressionModel", "LinearRegressionWithAGD",
            "LogisticRegressionModel", "LogisticRegressionWithAGD", "SVMModel", "SVMWithAGD",
@@ -27,4 +28,5 @@ __all__ = ["GeneralizedLinearAlgorithm", "GeneralizedLinearModel", "LinearRegres
            "SimpleUpdater", "SquaredL2Updater", "Updater", "bf16_to_f32", "build", "exported_symbols", "run_with_stats",
            "DEFAULT_SPLIT_SEED", "split_bounds", "MultivariateStatisticalSummary", "Statistics", "StandardScaler",
            "StandardScalerModel", "physical_model", "physical_projection", "BinaryClassificationMetrics", "RowMatrix",
-           "SingularValueDecomposition", "KMeans", "KMeansModel", "LocalKMeans"]
+           "SingularValueDecomposition", "KMeans", "KMeansModel", "LocalKMeans", "NaiveBayes", "NaiveBayesModel",
+           "MulticlassMetrics"]

@@ -28,6 +28,8 @@ BIN_POS, BIN_NEG, BIN_NAN, BIN_AUROC, BIN_AUPR, BIN_N = range(6)
  COLSTAT_N) = range(9)
 # agd_gramian: the largest agd_dim(h) it takes (AGD_GRAMIAN_MAX_DIM; beyond it the call fails and allocates nothing)
 GRAMIAN_MAX_DIM = 8192
+# agd_class_sums / agd_linear_confusion: the most class labels they take (AGD_MAX_CLASSES)
+MAX_CLASSES = 1024
 
 
 class Params(C.Structure):
@@ -128,6 +130,12 @@ _SIGNATURES = {
     "agd_kmeans_costs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_double)]),
     "agd_kmeans_sample": (C.c_int, [C.c_void_p, C.c_uint64, C.c_double, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
                                     C.POINTER(C.c_int64)]),
+    "agd_label_classes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
+                                    C.POINTER(C.c_int64)]),
+    "agd_class_sums": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]),
+    "agd_linear_argmax": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                    C.c_void_p]),
+    "agd_linear_confusion": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "agd_set_row_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "agd_row_filter_mask": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]),
     "agd_set_feature_transform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

@@ -105,6 +105,7 @@ enum KmBuf {
   kKmPart,                // per-piece sums | per-piece residuals | column residuals
   kKmPayload,             // [sums k x md | counts k | cost], exchanged over the world
   kKmRows,                // sampled rows, this device's at its rank's block of the world's
+  kKmClasses,             // agd_class_sums / agd_linear_confusion: the class labels (doubles) | confusion counts (u64)
   kKmBufs
 };
 constexpr size_t kBinMiscCounters = 8 * 256 * sizeof(unsigned), kBinMiscRuns = kBinMiscCounters + 8,
@@ -2019,6 +2020,7 @@ int agd_project(agd_handle *h, const double *B, int32_t k, const double *offset,
 }
 
 // ---------------------------------------------------------------- ranking metrics (rank.cu)
+static int bin_list(agd_handle *h, Dev &D, long long n, int64_t *len);
 // One shard: the key form of the scoring sweep (rows of the view, non-NaN margins), the radix sort and the run-length reduce
 // into this device's curve (D.bin[kBinList], *len records); *nan = rows of the view whose margin is NaN.
 static int bin_local(agd_handle *h, Dev &D, double intercept, int64_t *len, int64_t *nan) {
@@ -2039,8 +2041,14 @@ static int bin_local(agd_handle *h, Dev &D, double intercept, int64_t *len, int6
   unsigned cnt[2];
   CK(cudaMemcpyAsync(cnt, counters, sizeof cnt, cudaMemcpyDeviceToHost, D.st));
   CK(cudaStreamSynchronize(D.st));
-  const long long n = cnt[0];
   *nan = cnt[1];
+  return bin_list(h, D, cnt[0], len);
+}
+
+// The n keys and 1-byte values in D.bin[kBinKeys0] / [kBinVals0] sorted and reduced into this device's list (D.bin[kBinList],
+// *len records)
+static int bin_list(agd_handle *h, Dev &D, long long n, int64_t *len) {
+  char *misc = (char *)D.bin[kBinMisc];
   if (ensure_bin(h, D, kBinTiles, std::max(bin_sort_tile_words(n) * sizeof(unsigned), bin_runs_tile_words(n) * sizeof(long long))) ||
       ensure_bin(h, D, kBinList, (n > 0 ? (size_t)n : 1) * sizeof(BinRec)))
     return 1;
@@ -2185,34 +2193,45 @@ int agd_binary_curve(agd_handle *h, const double *w, double intercept, int64_t c
 // ---------------------------------------------------------------- clustering (kmeans.cu)
 // The centres as the kernels read them, built once on the host for every device: C [k][md] in the internal width md = d + bias
 // (zeros on padded columns), B [round_up(d, 16)][kp] = (s o C)^T zero-padded, cb = the bias entries, cn = ||c_j||^2 added over
-// the columns in order.
+// the columns in order.  With an offset (agd_linear_*: the rows of W as centres, kKmLinear scores) cn = the offset and C is
+// not built.
 struct KmCentres {
   int32_t k = 0, kp = 0, md = 0;
   std::vector<double> buf;   // B | cb | cn | C
   size_t nB = 0;
 };
-static int km_centres(agd_handle *h, const char *what, const double *centers, int32_t k, KmCentres &c) {
+static int km_centres(agd_handle *h, const char *what, const double *centers, int32_t k, KmCentres &c,
+                      const double *offset = nullptr) {
   if (h->d <= 0) return fail(h, "no shard loaded (call agd_load_dense / agd_load_csr / agd_generate first)");
-  if (k < 1) return fail(h, "%s: k = %d centres (at least 1)", what, k);
+  const bool linear = offset != nullptr;
+  if (k < 1) return fail(h, linear ? "%s: C = %d classes (at least 1)" : "%s: k = %d centres (at least 1)", what, k);
   if (!centers) return fail(h, "NULL argument");
   for (const Dev &D : h->devs)
     if (D.sh.rows >= (int64_t)1 << 31) return fail(h, "%s: %lld rows on device %d (at most 2^31 - 1)", what, (long long)D.sh.rows, D.ordinal);
   const int32_t du = h->d_user, d = h->d, b = h->tf_bias, Dx = du + b;
   for (size_t q = 0; q < (size_t)k * Dx; ++q)
-    if (!std::isfinite(centers[q])) return fail(h, "%s: centre %zu, feature %zu = %g is not finite", what, q / Dx, q % Dx, centers[q]);
+    if (!std::isfinite(centers[q]))
+      return fail(h, linear ? "%s: W[%zu][%zu] = %g is not finite" : "%s: centre %zu, feature %zu = %g is not finite", what, q / Dx,
+                  q % Dx, centers[q]);
+  if (linear)
+    for (int32_t j = 0; j < k; ++j)
+      if (!std::isfinite(offset[j])) return fail(h, "%s: offset[%d] = %g is not finite", what, j, offset[j]);
   const int32_t tc = project_tile_cols(k), bd = (d + 15) / 16 * 16;
   c.k = k; c.kp = (k + tc - 1) / tc * tc; c.md = d + b;
   c.nB = (size_t)bd * c.kp;
-  c.buf.assign(c.nB + 2 * (size_t)c.kp + (size_t)k * c.md, 0.0);
+  c.buf.assign(c.nB + 2 * (size_t)c.kp + (linear ? 0 : (size_t)k * c.md), 0.0);
   double *B = c.buf.data(), *cb = B + c.nB, *cn = cb + c.kp, *C = cn + c.kp;
   for (int32_t j = 0; j < k; ++j) {
     const double *src = centers + (size_t)j * Dx;
-    double *cj = C + (size_t)j * c.md;
-    for (int32_t l = 0; l < du; ++l) {
-      cj[l] = src[l];
-      B[(size_t)l * c.kp + j] = h->tf_scale ? h->tf_scale_host[(size_t)l] * src[l] : src[l];
+    for (int32_t l = 0; l < du; ++l) B[(size_t)l * c.kp + j] = h->tf_scale ? h->tf_scale_host[(size_t)l] * src[l] : src[l];
+    if (b) cb[j] = src[du];
+    if (linear) {
+      cn[j] = offset[j];
+      continue;
     }
-    if (b) cb[j] = cj[d] = src[du];
+    double *cj = C + (size_t)j * c.md;
+    for (int32_t l = 0; l < du; ++l) cj[l] = src[l];
+    if (b) cj[d] = src[du];
     double n = 0.0;
     for (int32_t l = 0; l < c.md; ++l) n += cj[l] * cj[l];
     cn[j] = n;
@@ -2220,27 +2239,33 @@ static int km_centres(agd_handle *h, const char *what, const double *centers, in
   return 0;
 }
 
-// D's arguments for the rows [0, rows) of its shard, the centres uploaded
-static int km_args(agd_handle *h, Dev &D, const KmCentres &c, KmeansArgs &a) {
+// D's arguments for the rows [0, rows) of its shard in the view's feature space (no centres)
+static int km_data(agd_handle *h, Dev &D, KmeansArgs &a) {
   const Shard &s = D.sh;
   CK(cudaSetDevice(D.ordinal));
-  if (ensure_km(h, D, kKmCentres, c.buf.size() * sizeof(double))) return 1;
-  double *dev = (double *)D.km[kKmCentres];
-  CK(cudaMemcpyAsync(dev, c.buf.data(), c.buf.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
   if (h->filt.n && ensure_view_bits(h, D)) return 1;
   a = KmeansArgs();
   if (s.csr) { a.rowptr = s.rowptr; a.idx = s.idx; a.val = s.val; }
   else a.X = s.X;
-  a.rows = s.rows; a.d = h->d; a.md = c.md; a.bias = h->tf_bias; a.scale = h->scale_of(D);
+  a.rows = s.rows; a.d = h->d; a.md = h->d + h->tf_bias; a.bias = h->tf_bias; a.scale = h->scale_of(D);
   a.view_bits = h->filt.n ? D.view_bits : nullptr;
-  a.k = c.k; a.kp = c.kp;
-  a.B = dev; a.cb = dev + c.nB; a.cn = a.cb + c.kp; a.C = a.cn + c.kp;
   a.stream = D.st;
   return 0;
 }
 
-// centres of rows [a.row0, a.row0 + a.rows) into D.km[kKmCluster]
-static int km_assign(agd_handle *h, Dev &D, KmeansArgs &a) {
+// ... and the centres uploaded
+static int km_args(agd_handle *h, Dev &D, const KmCentres &c, KmeansArgs &a) {
+  if (km_data(h, D, a)) return 1;
+  if (ensure_km(h, D, kKmCentres, c.buf.size() * sizeof(double))) return 1;
+  double *dev = (double *)D.km[kKmCentres];
+  CK(cudaMemcpyAsync(dev, c.buf.data(), c.buf.size() * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  a.k = c.k; a.kp = c.kp;
+  a.B = dev; a.cb = dev + c.nB; a.cn = a.cb + c.kp; a.C = a.cn + c.kp;
+  return 0;
+}
+
+// centres (kKmLinear: argmax classes) of rows [a.row0, a.row0 + a.rows) into D.km[kKmCluster]
+static int km_assign(agd_handle *h, Dev &D, KmeansArgs &a, int score_mode = kKmDistance) {
   const size_t r1 = a.rows > 0 ? (size_t)a.rows : 1;
   if (ensure_km(h, D, kKmCluster, r1 * sizeof(int32_t))) return 1;
   a.cluster = (int32_t *)D.km[kKmCluster];
@@ -2250,16 +2275,15 @@ static int km_assign(agd_handle *h, Dev &D, KmeansArgs &a) {
     a.tile_score = (double *)D.km[kKmTiles];
     a.tile_idx = (int32_t *)(a.tile_score + tiles * r1);
   }
-  CK(kmeans_assign_launch(a, D.sh.elem_bytes, D.sm_count));
+  CK(kmeans_assign_launch(a, D.sh.elem_bytes, D.sm_count, score_mode));
   return 0;
 }
 
-// One device's share of a step: the payload [sums k x md | counts k | cost] in D.km[kKmPayload]
-static int km_step_device(agd_handle *h, Dev &D, const KmCentres &c) {
-  KmeansArgs a;
-  if (km_args(h, D, c, a) || km_assign(h, D, a)) return 1;
+// One device's sums over the rows a.cluster assigns to a.k groups (-1: none): the payload [sums k x md | counts k | cost] in
+// D.km[kKmPayload], cost = the residuals to the centres (kKmResidual) or the count of entries not >= 0 (kKmNegatives)
+static int km_sums_device(agd_handle *h, Dev &D, const KmeansArgs &a, int sums_mode) {
   const Shard &s = D.sh;
-  const int32_t k = c.k, md = c.md;
+  const int32_t k = a.k, md = a.md;
   const size_t P = (size_t)k * md + k + 1, r1 = s.rows > 0 ? (size_t)s.rows : 1;
   if (ensure_km(h, D, kKmPayload, P * sizeof(double)) || ensure_km(h, D, kKmMisc, 8 * 256 * sizeof(unsigned) + ((size_t)k + 1) * 8) ||
       ensure_km(h, D, kKmKeys0, 8 * r1) || ensure_km(h, D, kKmVals0, 4 * r1))
@@ -2273,7 +2297,7 @@ static int km_step_device(agd_handle *h, Dev &D, const KmCentres &c) {
   CK(cudaMemsetAsync(counts, 0, ((size_t)k + 1) * 8, D.st));
   CK(kmeans_keys_launch(a.cluster, s.rows, k, keys[0], (uint32_t *)vals[0], counts, D.st));
   if (s.csr) {
-    CK(kmeans_sums_csr_launch(a, s.elem_bytes, D.sm_count, pay));
+    CK(kmeans_sums_csr_launch(a, s.elem_bytes, D.sm_count, pay, sums_mode));
   } else if (s.rows > 0) {
     // rows sorted stably by centre, then each centre's rows in pieces of kKmPiece, every piece's columns added in sorted order
     if (ensure_km(h, D, kKmKeys1, 8 * r1) || ensure_km(h, D, kKmVals1, 4 * r1) ||
@@ -2308,12 +2332,18 @@ static int km_step_device(agd_handle *h, Dev &D, const KmCentres &c) {
     if (np) CK(cudaMemcpyAsync(pc, pcl.data(), pcl.size() * 4, cudaMemcpyHostToDevice, D.st));
     CK(cudaMemcpyAsync(pf, pfirst.data(), pfirst.size() * 4, cudaMemcpyHostToDevice, D.st));
     double *part = (double *)D.km[kKmPart], *pres = part + (size_t)np * md, *colres = pres + (size_t)np * md;
-    CK(kmeans_sums_dense_launch(a, s.elem_bytes, (const uint32_t *)vals[which], ps, pc, np, part, pres));
+    CK(kmeans_sums_dense_launch(a, s.elem_bytes, (const uint32_t *)vals[which], ps, pc, np, part, pres, sums_mode));
     CK(kmeans_sums_reduce_launch(part, pres, pf, np, k, md, pay, colres, D.st));
     CK(cudaStreamSynchronize(D.st));   // pstart / pcl / pfirst live on this stack frame until the copies ran
   }
   CK(kmeans_counts_launch(counts, k, md, pay, D.st));
   return 0;
+}
+
+// One device's share of a step: every row of the view assigned to its centre, then the sums
+static int km_step_device(agd_handle *h, Dev &D, const KmCentres &c) {
+  KmeansArgs a;
+  return km_args(h, D, c, a) || km_assign(h, D, a) || km_sums_device(h, D, a, kKmResidual);
 }
 
 int agd_kmeans_step(agd_handle *h, const double *centers, int32_t k, double *sums_out, double *counts_out, double *cost_out) {
@@ -2494,6 +2524,163 @@ int agd_kmeans_sample(agd_handle *h, uint64_t seed, double factor, int32_t weigh
       model_values(h, z, 1.0, rows_out + o * Dx);
       if (draws_out) draws_out[o] = z[md];
     }
+  return 0;
+}
+
+// ---------------------------------------------------------------- classification (classify.cu, and the k-means kernels)
+int agd_label_classes(agd_handle *h, int64_t capacity, double *labels_out, int64_t *counts_out, int64_t *n_out,
+                      int64_t *nan_out) {
+  if (check_ready(h)) return 1;
+  if (!n_out || !nan_out) return fail(h, "NULL argument");
+  if (capacity < 0) return fail(h, "capacity must be >= 0 (got %lld)", (long long)capacity);
+  if (capacity > 0 && (!labels_out || !counts_out)) return fail(h, "NULL argument");
+  const int nd = (int)h->devs.size();
+  std::vector<int64_t> len((size_t)nd), nan((size_t)nd);
+  for (int i = 0; i < nd; ++i) {
+    Dev &D = h->devs[i];
+    const int64_t rows = D.sh.rows;
+    CK(cudaSetDevice(D.ordinal));
+    if (rows >= (int64_t)1 << 31) return fail(h, "agd_label_classes: %lld rows on device %d (at most 2^31 - 1)", (long long)rows, D.ordinal);
+    const size_t r1 = rows > 0 ? (size_t)rows : 1;
+    if (ensure_bin(h, D, kBinMisc, kBinMiscAll + 16 * (size_t)h->world + 8 * ((size_t)h->world + 1)) ||
+        ensure_bin(h, D, kBinKeys0, 8 * r1) || ensure_bin(h, D, kBinKeys1, 8 * r1) || ensure_bin(h, D, kBinVals0, r1) ||
+        ensure_bin(h, D, kBinVals1, r1))
+      return 1;
+    if (h->filt.n && ensure_view_bits(h, D)) return 1;
+    unsigned *counters = (unsigned *)((char *)D.bin[kBinMisc] + kBinMiscCounters);
+    CK(cudaMemsetAsync(counters, 0, 2 * sizeof(unsigned), D.st));
+    CK(label_keys_launch(D.sh.labels, h->filt.n ? D.view_bits : nullptr, rows, (unsigned long long *)D.bin[kBinKeys0],
+                         (uint8_t *)D.bin[kBinVals0], counters, D.st));
+    unsigned cnt[2];
+    CK(cudaMemcpyAsync(cnt, counters, sizeof cnt, cudaMemcpyDeviceToHost, D.st));
+    CK(cudaStreamSynchronize(D.st));
+    nan[(size_t)i] = cnt[1];
+    if (bin_list(h, D, cnt[0], &len[(size_t)i])) return 1;
+  }
+  Dev &D0 = h->devs[0];
+  BinRec *list = (BinRec *)D0.bin[kBinList];
+  int64_t K = len[0], nans = nan[0];
+  if (h->world > 1 && bin_world(h, len, nan, &list, &K, &nans)) return 1;
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<BinRec> host;
+  if (K > 0 && capacity >= K) {
+    host.resize((size_t)K);
+    CK(cudaMemcpyAsync(host.data(), list, (size_t)K * sizeof(BinRec), cudaMemcpyDeviceToHost, D0.st));
+  }
+  if (sync_all(h)) return 1;
+  *n_out = K;
+  *nan_out = nans;
+  for (size_t k = 0; k < host.size(); ++k) {   // tp holds the cumulative count: every key came with the value 1
+    labels_out[k] = label_of_key(host[k].key);
+    counts_out[k] = host[k].tp - (k > 0 ? host[k - 1].tp : 0);
+  }
+  return 0;
+}
+
+// The C class labels uploaded to D.km[kKmClasses], extra_bytes more behind them
+static int cls_upload(agd_handle *h, Dev &D, const double *labels, int32_t C, size_t extra_bytes) {
+  if (ensure_km(h, D, kKmClasses, (size_t)C * sizeof(double) + extra_bytes)) return 1;
+  CK(cudaMemcpyAsync(D.km[kKmClasses], labels, (size_t)C * sizeof(double), cudaMemcpyHostToDevice, D.st));
+  return 0;
+}
+// C ascending, distinct, non-NaN class labels, at most AGD_MAX_CLASSES
+static int cls_check(agd_handle *h, const char *what, const double *labels, int32_t C) {
+  if (C < 1 || C > AGD_MAX_CLASSES) return fail(h, "%s: %d classes (1 to %d)", what, C, (int)AGD_MAX_CLASSES);
+  if (!labels) return fail(h, "NULL argument");
+  for (int32_t c = 0; c < C; ++c) {
+    if (labels[c] != labels[c]) return fail(h, "%s: labels[%d] is NaN", what, c);
+    if (c > 0 && !(labels[c - 1] < labels[c]))
+      return fail(h, "%s: labels must ascend strictly (labels[%d] = %g, labels[%d] = %g)", what, c - 1, labels[c - 1], c, labels[c]);
+  }
+  return 0;
+}
+
+int agd_class_sums(agd_handle *h, const double *labels, int32_t C, double *sums_out, double *counts_out, double *negative_out) {
+  if (check_ready(h) || cls_check(h, "agd_class_sums", labels, C)) return 1;
+  if (!sums_out || !counts_out || !negative_out) return fail(h, "NULL argument");
+  for (const Dev &D : h->devs)
+    if (D.sh.rows >= (int64_t)1 << 31)
+      return fail(h, "agd_class_sums: %lld rows on device %d (at most 2^31 - 1)", (long long)D.sh.rows, D.ordinal);
+  for (Dev &D : h->devs) {
+    KmeansArgs a;
+    if (km_data(h, D, a) || cls_upload(h, D, labels, C, 0)) return 1;
+    const size_t r1 = D.sh.rows > 0 ? (size_t)D.sh.rows : 1;
+    if (ensure_km(h, D, kKmCluster, r1 * sizeof(int32_t))) return 1;
+    a.k = C;
+    a.cluster = (int32_t *)D.km[kKmCluster];
+    CK(label_class_launch(D.sh.labels, a.view_bits, D.sh.rows, (const double *)D.km[kKmClasses], C, a.cluster, D.st));
+    if (km_sums_device(h, D, a, kKmNegatives)) return 1;
+  }
+  const int32_t md = h->d + h->tf_bias;
+  const size_t P = (size_t)C * md + C + 1;
+  if (world_reduce(h, [&](size_t i) { return (double *)h->devs[i].km[kKmPayload]; }, P, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  std::vector<double> r(P);
+  CK(cudaMemcpyAsync(r.data(), D0.km[kKmPayload], P * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
+  const int32_t Dx = h->d_user + h->tf_bias;
+  for (int32_t c = 0; c < C; ++c) {
+    model_values(h, &r[(size_t)c * md], 1.0, sums_out + (size_t)c * Dx);
+    counts_out[c] = r[(size_t)C * md + c];
+  }
+  *negative_out = r[P - 1];
+  return 0;
+}
+
+int agd_linear_argmax(agd_handle *h, int32_t dev, const double *W, int32_t C, const double *offset, int64_t row0, int64_t rows,
+                      int32_t *class_out) {
+  if (!h) return 1;
+  if (dev < 0 || dev >= (int)h->devs.size()) return fail(h, "bad local device index %d", dev);
+  if (!offset) return fail(h, "NULL argument");
+  KmCentres c;
+  if (km_centres(h, "agd_linear_argmax", W, C, c, offset)) return 1;
+  Dev &D = h->devs[dev];
+  if (row0 < 0 || rows < 0 || rows > D.sh.rows - row0)
+    return fail(h, "row range [%lld, %lld + %lld) lies outside the %lld rows of device %d", (long long)row0, (long long)row0,
+                (long long)rows, (long long)D.sh.rows, dev);
+  if (rows > 0 && !class_out) return fail(h, "NULL argument");
+  if (rows == 0) return 0;
+  KmeansArgs a;
+  if (km_args(h, D, c, a)) return 1;
+  // a row's class depends on the row only, so the range is scored in chunks
+  const int64_t chunk = rows < (int64_t)(1 << 22) ? rows : (int64_t)(1 << 22);
+  for (int64_t r0 = 0; r0 < rows; r0 += chunk) {
+    a.row0 = row0 + r0;
+    a.rows = rows - r0 < chunk ? rows - r0 : chunk;
+    if (km_assign(h, D, a, kKmLinear)) return 1;
+    CK(cudaMemcpyAsync(class_out + r0, a.cluster, (size_t)a.rows * sizeof(int32_t), cudaMemcpyDeviceToHost, D.st));
+    CK(cudaStreamSynchronize(D.st));   // the buffer is reused
+  }
+  return 0;
+}
+
+int agd_linear_confusion(agd_handle *h, const double *W, int32_t C, const double *offset, const double *labels, int32_t L,
+                         double *counts_out) {
+  if (check_ready(h) || cls_check(h, "agd_linear_confusion", labels, L)) return 1;
+  if (!offset || !counts_out) return fail(h, "NULL argument");
+  if (C > AGD_MAX_CLASSES) return fail(h, "agd_linear_confusion: C = %d classes (at most %d)", C, (int)AGD_MAX_CLASSES);
+  KmCentres c;
+  if (km_centres(h, "agd_linear_confusion", W, C, c, offset)) return 1;
+  const size_t n = (size_t)L * C;
+  for (Dev &D : h->devs) {
+    KmeansArgs a;
+    if (km_args(h, D, c, a) || km_assign(h, D, a, kKmLinear)) return 1;
+    const size_t lb = ((size_t)L * sizeof(double) + 15) / 16 * 16;
+    if (cls_upload(h, D, labels, L, lb - (size_t)L * sizeof(double) + n * 8) ||
+        ensure_km(h, D, kKmPayload, n * sizeof(double)))
+      return 1;
+    unsigned long long *cnt = (unsigned long long *)((char *)D.km[kKmClasses] + lb);
+    CK(cudaMemsetAsync(cnt, 0, n * 8, D.st));
+    CK(label_confusion_launch(D.sh.labels, a.cluster, D.sh.rows, (const double *)D.km[kKmClasses], L, C, cnt, D.sm_count, D.st));
+    // the counts as doubles: kmeans_counts_launch with k = L C and md = 0 writes out[j] = counts[j]
+    CK(kmeans_counts_launch(cnt, (int32_t)n, 0, (double *)D.km[kKmPayload], D.st));
+  }
+  if (world_reduce(h, [&](size_t i) { return (double *)h->devs[i].km[kKmPayload]; }, n, kXchgSum)) return 1;
+  Dev &D0 = h->devs[0];
+  CK(cudaSetDevice(D0.ordinal));
+  CK(cudaMemcpyAsync(counts_out, D0.km[kKmPayload], n * sizeof(double), cudaMemcpyDeviceToHost, D0.st));
+  if (sync_all(h)) return 1;
   return 0;
 }
 

@@ -336,6 +336,11 @@ cudaError_t project_csr_launch(const ProjectArgs &a, int elem_bytes, int sm_coun
 // A row's centre is the lowest index j minimising the score ||c_j||^2 - 2 (x . B_j + cb_j) with B_lj = s_l c_jl: the cross term
 // is the projection's fp64 sum (pj_tile.cuh, or a CSR row's stored entries in stored order); a NaN score never wins.
 constexpr int kKmPiece = 4096;      // sorted rows per piece of the dense sums
+// Compile-time modes of the k-means kernels.  Score: kKmDistance is k-means' own; kKmLinear scores class j as
+// -(offset_j + x . B_j + cb_j) with the offset in the cn slot, so the lowest (score, j) is the linear model's argmax (agd_linear_*).
+// Sums: kKmResidual adds the residuals to the centres; kKmNegatives counts the entries that are not >= 0 (agd_class_sums).
+enum { kKmDistance = 0, kKmLinear = 1 };
+enum { kKmResidual = 0, kKmNegatives = 1 };
 struct KmeansArgs {
   const void *X = nullptr;          // dense shard (fp32 / fp64 / bf16), row-major, ld == d
   const int64_t *rowptr = nullptr;  // CSR shard (fp32 / fp64 values)
@@ -357,7 +362,7 @@ struct KmeansArgs {
   int32_t *tile_idx = nullptr;      // ... the best of each 128-column tile, when kp > 128
   cudaStream_t stream = nullptr;
 };
-cudaError_t kmeans_assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count);
+cudaError_t kmeans_assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count, int score_mode = kKmDistance);
 // Exact residual sum_l (z_l - c_l)^2 of each row of the range to its cluster's centre (CSR: ||c||^2 + sum over the stored
 // entries of (z_l - c_l)^2 - c_l^2, the bias column counted as stored).  dist != nullptr: dist[i] (NaN outside the view).
 // Else delta[i] = the residual, or with keep the smaller of it and delta[i] (a NaN residual never replaces delta[i]), and the
@@ -369,15 +374,18 @@ cudaError_t kmeans_dist_launch(const KmeansArgs &a, int elem_bytes, int sm_count
 cudaError_t kmeans_keys_launch(const int32_t *cluster, long long rows, int32_t k, unsigned long long *keys, uint32_t *vals,
                                unsigned long long *counts, cudaStream_t st);
 // Dense sums over pieces of the rows sorted by cluster: piece p is sorted positions [pstart[p], pstart[p + 1]) of cluster
-// pcl[p]; part[p][c] = sum z_c, pres[p][c] = sum (z_c - C[pcl[p]][c])^2, each a sequential fp64 sum in sorted order.
+// pcl[p]; part[p][c] = sum z_c, pres[p][c] = sum (z_c - C[pcl[p]][c])^2 (kKmNegatives: the count of z_c not >= 0), each a
+// sequential fp64 sum in sorted order.
 cudaError_t kmeans_sums_dense_launch(const KmeansArgs &a, int elem_bytes, const uint32_t *order, const long long *pstart,
-                                     const int32_t *pcl, long long npieces, double *part, double *pres);
+                                     const int32_t *pcl, long long npieces, double *part, double *pres,
+                                     int sums_mode = kKmResidual);
 // out[j][c] = the pieces pfirst[j] .. pfirst[j + 1] - 1 of part added in order; out[k md + k] = the cost, pres added over the
 // pieces in order per column, then over the columns in order
 cudaError_t kmeans_sums_reduce_launch(const double *part, const double *pres, const int32_t *pfirst, long long npieces,
                                       int32_t k, int32_t md, double *out, double *colres, cudaStream_t st);
-// CSR: out[j][c] += z_c and out[k md + k] += the row's residual, by fp64 RED.ADD (out zeroed by the caller)
-cudaError_t kmeans_sums_csr_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *out);
+// CSR: out[j][c] += z_c and out[k md + k] += the row's residual (kKmNegatives: its stored z_c not >= 0), by fp64 RED.ADD (out
+// zeroed by the caller)
+cudaError_t kmeans_sums_csr_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *out, int sums_mode = kKmResidual);
 // out[k md + j] = counts[j], j < k
 cudaError_t kmeans_counts_launch(const unsigned long long *counts, int32_t k, int32_t md, double *out, cudaStream_t st);
 // k-means sampling: row r of the view is kept iff u < factor delta[r] (delta = 1 when delta == nullptr), u = the row's draw of
@@ -388,6 +396,22 @@ cudaError_t kmeans_sample_bits_launch(const KmeansArgs &a, unsigned long long se
 // the kept rows, compacted through tile_base (project_scan_launch of bits): out[o] = [z (md doubles) | u]
 cudaError_t kmeans_sample_rows_launch(const KmeansArgs &a, int elem_bytes, unsigned long long seed, long long row_base,
                                       const uint32_t *bits, const long long *tile_base, double *out, int sm_count);
+
+// ---------------------------------------------------------------- classification (classify.cu, agd_label_classes / agd_class_sums /
+// agd_linear_confusion).  Labels are compared by value (-0.0 == 0.0); `classes` are C ascending non-NaN doubles.
+// The label key of a row: ascending in the label, -0.0 keyed as 0.0 (label_of_key inverts it, giving +0.0)
+__host__ __device__ inline unsigned long long label_key(double y) { return margin_key(-y); }
+__host__ __device__ inline double label_of_key(unsigned long long k) { return 0.0 - margin_of_key(k); }
+// For every row of [0, rows) in the view (view_bits, nullptr: every row): a non-NaN label appends (label_key, 1) to keys / ones
+// (compacted, counters[0] = their number); a NaN label adds 1 to counters[1].  counters zeroed by the caller.
+cudaError_t label_keys_launch(const double *labels, const uint32_t *view_bits, long long rows, unsigned long long *keys,
+                              uint8_t *ones, unsigned *counters, cudaStream_t st);
+// cls[i] = the index of labels[i] in classes, -1 for a label that is none of them (NaN included) or a row outside the view
+cudaError_t label_class_launch(const double *labels, const uint32_t *view_bits, long long rows, const double *classes,
+                               int32_t C, int32_t *cls, cudaStream_t st);
+// counts[l][c] += the rows with labels[i] == classes[l] and pred[i] == c >= 0 (counts: L x C zeroed u64; C <= 12,288)
+cudaError_t label_confusion_launch(const double *labels, const int32_t *pred, long long rows, const double *classes, int32_t L,
+                                   int32_t C, unsigned long long *counts, int sm_count, cudaStream_t st);
 
 // out[i] = 1 if row row_base + i passes the filter, else 0 (agd_row_filter_mask; the kernels' own row_in_view())
 cudaError_t row_filter_mask_launch(const RowFilter *f, long long row_base, int64_t rows, uint8_t *out, cudaStream_t st);

@@ -30,8 +30,9 @@ __device__ __forceinline__ bool km_in_view(const uint32_t *bits, long long r) {
 __device__ __forceinline__ void km_take(double s, int j, double &bs, int &bj) {
   if (s < bs || (s == bs && j < bj)) { bs = s; bj = j; }
 }
-__device__ __forceinline__ double km_score(const KmeansArgs &a, int j, double acc) {
-  const double s = a.cn[j] - 2.0 * (acc + a.cb[j]);
+// kKmDistance: ||c_j||^2 - 2 (acc + cb_j); kKmLinear: -(offset_j + acc + cb_j), the offset in the cn slot (the argmax as an argmin)
+template <int MODE> __device__ __forceinline__ double km_score(const KmeansArgs &a, int j, double acc) {
+  const double s = MODE == kKmLinear ? -(a.cn[j] + acc + a.cb[j]) : a.cn[j] - 2.0 * (acc + a.cb[j]);
   return s != s ? kKmInf : s;
 }
 __device__ __forceinline__ void km_warp_min(double &bs, int &bj) {
@@ -53,7 +54,7 @@ template <typename T> __device__ __forceinline__ double km_z(const KmeansArgs &a
 }
 
 // Row tile rt0 + blockIdx.y (of the range), column tile blockIdx.x
-template <typename T, bool VEC, int BN>
+template <typename T, bool VEC, int BN, int MODE>
 __global__ void __launch_bounds__(kPjThreads, BN == 128 ? 1 : 2) kmeans_dense_kernel(const KmeansArgs a, const long long rt0) {
   using S = PjShape<BN>;
   extern __shared__ __align__(16) unsigned char pj_smem[];
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(kPjThreads, BN == 128 ? 1 : 2) kmeans_dense_ke
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int j = c0 + pj_frag_col<BN>(nt, 2 * h + e);
-          if (j < a.k) km_take(km_score(a, j, acc[mt][nt][2 * h + e]), j, bs[mt][h], bj[mt][h]);
+          if (j < a.k) km_take(km_score<MODE>(a, j, acc[mt][nt][2 * h + e]), j, bs[mt][h], bj[mt][h]);
         }
 #pragma unroll
       for (int off = 1; off < 4; off <<= 1)
@@ -130,7 +131,7 @@ __global__ void kmeans_tiles_kernel(const KmeansArgs a, int tiles) {
 
 // One warp per row of the range, lanes over centres in passes of 32 kKmCsrCols; every stored entry, in stored order, adds
 // x B[col, :] in fp64
-template <typename T>
+template <typename T, int MODE>
 __global__ void __launch_bounds__(kKmWarpThreads) kmeans_csr_kernel(const KmeansArgs a) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (long long)blockIdx.x * (kKmWarpThreads / 32) + (threadIdx.x >> 5);
@@ -161,7 +162,7 @@ __global__ void __launch_bounds__(kKmWarpThreads) kmeans_csr_kernel(const Kmeans
 #pragma unroll
       for (int q = 0; q < kKmCsrCols; ++q) {
         const int j = j0 + q * 32 + lane;
-        if (j < a.k) km_take(km_score(a, j, acc[q]), j, bs, bj);
+        if (j < a.k) km_take(km_score<MODE>(a, j, acc[q]), j, bs, bj);
       }
     }
     km_warp_min(bs, bj);
@@ -247,8 +248,9 @@ __global__ void kmeans_keys_kernel(const int32_t *__restrict__ cluster, long lon
   atomicAdd(counts + key, 1ull);
 }
 
-// Piece blockIdx.y, columns blockIdx.x kKmCols + threadIdx.x
-template <typename T>
+// Piece blockIdx.y, columns blockIdx.x kKmCols + threadIdx.x.  kKmResidual: pres = sum (z - c)^2; kKmNegatives: pres = the
+// entries that are not >= 0 (NaN included), and C is not read
+template <typename T, int MODE>
 __global__ void __launch_bounds__(kKmCols) kmeans_sums_dense_kernel(const KmeansArgs a, const uint32_t *__restrict__ order,
                                                                     const long long *__restrict__ pstart,
                                                                     const int32_t *__restrict__ pcl, double *part, double *pres) {
@@ -256,7 +258,7 @@ __global__ void __launch_bounds__(kKmCols) kmeans_sums_dense_kernel(const Kmeans
   const long long p = blockIdx.y;
   const int col = blockIdx.x * kKmCols + threadIdx.x;
   const long long q0 = pstart[p], q1 = pstart[p + 1];
-  const double c = col < a.md ? a.C[(size_t)pcl[p] * a.md + col] : 0.0;
+  const double c = MODE == kKmResidual && col < a.md ? a.C[(size_t)pcl[p] * a.md + col] : 0.0;
   double s = 0.0, e2 = 0.0;
   for (long long b = q0; b < q1; b += kKmCols) {
     const int n = q1 - b < kKmCols ? (int)(q1 - b) : kKmCols;
@@ -266,9 +268,14 @@ __global__ void __launch_bounds__(kKmCols) kmeans_sums_dense_kernel(const Kmeans
     if (col < a.md) {
 #pragma unroll 8
       for (int i = 0; i < n; ++i) {
-        const double z = km_z<T>(a, a.row0 + rows[i], col), e = z - c;
+        const double z = km_z<T>(a, a.row0 + rows[i], col);
         s += z;
-        e2 = fma(e, e, e2);
+        if (MODE == kKmNegatives) {
+          e2 += z >= 0.0 ? 0.0 : 1.0;
+        } else {
+          const double e = z - c;
+          e2 = fma(e, e, e2);
+        }
       }
     }
   }
@@ -302,7 +309,8 @@ __global__ void kmeans_cost_kernel(const double *colres, int32_t k, int32_t md, 
   out[(size_t)k * md + k] = s;
 }
 
-template <typename T>
+// kKmResidual: out[k md + k] += each row's residual; kKmNegatives: += the stored entries that are not >= 0 (NaN included)
+template <typename T, int MODE>
 __global__ void __launch_bounds__(kKmWarpThreads) kmeans_sums_csr_kernel(const KmeansArgs a, double *out) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (long long)blockIdx.x * (kKmWarpThreads / 32) + (threadIdx.x >> 5);
@@ -314,13 +322,15 @@ __global__ void __launch_bounds__(kKmWarpThreads) kmeans_sums_csr_kernel(const K
     const long long r = a.row0 + l;
     const long long k0 = __ldg(a.rowptr + r), k1 = __ldg(a.rowptr + r + 1);
     double *sj = out + (size_t)j * a.md;
+    double neg = 0.0;
     for (long long e = k0 + lane; e < k1; e += 32) {
       const int col = __ldg(a.idx + e);
       double x = (double)val[e];
       if (a.scale) x *= a.scale[col];
       atomicAdd(sj + col, x);
+      if (MODE == kKmNegatives) neg += x >= 0.0 ? 0.0 : 1.0;
     }
-    const double v = km_resid_csr<T>(a, r, j, lane);
+    const double v = MODE == kKmNegatives ? km_warp_sum(neg) : km_resid_csr<T>(a, r, j, lane);
     if (lane == 0) {
       if (a.bias) atomicAdd(sj + a.d, 1.0);
       atomicAdd(out + (size_t)a.k * a.md + a.k, v);
@@ -377,23 +387,23 @@ __global__ void __launch_bounds__(kKmWarpThreads) kmeans_sample_rows_kernel(cons
   }
 }
 
-template <typename T, bool VEC, int BN>
+template <typename T, bool VEC, int BN, int MODE>
 cudaError_t launch_dense(const KmeansArgs &a) {
-  return pj_launch_rows<T, BN>(kmeans_dense_kernel<T, VEC, BN>, a, a.rows, a.kp / BN, a.stream);
+  return pj_launch_rows<T, BN>(kmeans_dense_kernel<T, VEC, BN, MODE>, a, a.rows, a.kp / BN, a.stream);
 }
-template <typename T, int BN>
+template <typename T, int BN, int MODE>
 cudaError_t launch_dense_vec(const KmeansArgs &a) {
-  if ((size_t)a.d * sizeof(T) % 16 == 0) return launch_dense<T, true, BN>(a);
-  return launch_dense<T, false, BN>(a);
+  if ((size_t)a.d * sizeof(T) % 16 == 0) return launch_dense<T, true, BN, MODE>(a);
+  return launch_dense<T, false, BN, MODE>(a);
 }
-template <typename T>
+template <typename T, int MODE>
 cudaError_t launch_dense_t(const KmeansArgs &a) {
   cudaError_t e;
   switch (project_tile_cols(a.k)) {
-    case 16: e = launch_dense_vec<T, 16>(a); break;
-    case 32: e = launch_dense_vec<T, 32>(a); break;
-    case 64: e = launch_dense_vec<T, 64>(a); break;
-    default: e = launch_dense_vec<T, 128>(a); break;
+    case 16: e = launch_dense_vec<T, 16, MODE>(a); break;
+    case 32: e = launch_dense_vec<T, 32, MODE>(a); break;
+    case 64: e = launch_dense_vec<T, 64, MODE>(a); break;
+    default: e = launch_dense_vec<T, 128, MODE>(a); break;
   }
   if (e != cudaSuccess || a.kp <= 128) return e;
   kmeans_tiles_kernel<<<(unsigned)((a.rows + 255) / 256), 256, 0, a.stream>>>(a, a.kp / 128);
@@ -412,22 +422,29 @@ template <typename Kern> cudaError_t warp_grid(Kern kern, long long rows, int sm
   return cudaSuccess;
 }
 
-}  // namespace
-
-cudaError_t kmeans_assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count) {
+template <int MODE>
+cudaError_t assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count) {
   if (a.rows <= 0) return cudaSuccess;
   if (a.rowptr) {
     if (elem_bytes != 4 && elem_bytes != 8) return cudaErrorInvalidValue;
-    auto kern = elem_bytes == 8 ? kmeans_csr_kernel<double> : kmeans_csr_kernel<float>;
+    auto kern = elem_bytes == 8 ? kmeans_csr_kernel<double, MODE> : kmeans_csr_kernel<float, MODE>;
     unsigned grid = 0;
     cudaError_t e = warp_grid(kern, a.rows, sm_count, &grid);
     if (e != cudaSuccess) return e;
     kern<<<grid, kKmWarpThreads, 0, a.stream>>>(a);
     return cudaGetLastError();
   }
-  if (elem_bytes == 2) return launch_dense_t<__nv_bfloat16>(a);
-  if (elem_bytes == 4) return launch_dense_t<float>(a);
-  if (elem_bytes == 8) return launch_dense_t<double>(a);
+  if (elem_bytes == 2) return launch_dense_t<__nv_bfloat16, MODE>(a);
+  if (elem_bytes == 4) return launch_dense_t<float, MODE>(a);
+  if (elem_bytes == 8) return launch_dense_t<double, MODE>(a);
+  return cudaErrorInvalidValue;
+}
+
+}  // namespace
+
+cudaError_t kmeans_assign_launch(const KmeansArgs &a, int elem_bytes, int sm_count, int score_mode) {
+  if (score_mode == kKmLinear) return assign_launch<kKmLinear>(a, elem_bytes, sm_count);
+  if (score_mode == kKmDistance) return assign_launch<kKmDistance>(a, elem_bytes, sm_count);
   return cudaErrorInvalidValue;
 }
 
@@ -457,8 +474,10 @@ cudaError_t kmeans_keys_launch(const int32_t *cluster, long long rows, int32_t k
 }
 
 cudaError_t kmeans_sums_dense_launch(const KmeansArgs &a, int elem_bytes, const uint32_t *order, const long long *pstart,
-                                     const int32_t *pcl, long long npieces, double *part, double *pres) {
+                                     const int32_t *pcl, long long npieces, double *part, double *pres, int sums_mode) {
   if (npieces <= 0) return cudaSuccess;
+  if (sums_mode != kKmResidual && sums_mode != kKmNegatives) return cudaErrorInvalidValue;
+  const bool neg = sums_mode == kKmNegatives;
   const unsigned cx = (unsigned)((a.md + kKmCols - 1) / kKmCols);
   for (long long p0 = 0; p0 < npieces; p0 += kPjMaxGridY) {
     const long long n = npieces - p0 < kPjMaxGridY ? npieces - p0 : kPjMaxGridY;
@@ -467,9 +486,12 @@ cudaError_t kmeans_sums_dense_launch(const KmeansArgs &a, int elem_bytes, const 
     const int32_t *pc = pcl + p0;
     double *pa = part + (size_t)p0 * a.md, *pr = pres + (size_t)p0 * a.md;
     switch (elem_bytes) {
-      case 2: kmeans_sums_dense_kernel<__nv_bfloat16><<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
-      case 4: kmeans_sums_dense_kernel<float><<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
-      case 8: kmeans_sums_dense_kernel<double><<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
+      case 2: (neg ? kmeans_sums_dense_kernel<__nv_bfloat16, kKmNegatives> : kmeans_sums_dense_kernel<__nv_bfloat16, kKmResidual>)
+                  <<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
+      case 4: (neg ? kmeans_sums_dense_kernel<float, kKmNegatives> : kmeans_sums_dense_kernel<float, kKmResidual>)
+                  <<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
+      case 8: (neg ? kmeans_sums_dense_kernel<double, kKmNegatives> : kmeans_sums_dense_kernel<double, kKmResidual>)
+                  <<<g, kKmCols, 0, a.stream>>>(a, order, ps, pc, pa, pr); break;
       default: return cudaErrorInvalidValue;
     }
     cudaError_t e = cudaGetLastError();
@@ -486,10 +508,13 @@ cudaError_t kmeans_sums_reduce_launch(const double *part, const double *pres, co
   return cudaGetLastError();
 }
 
-cudaError_t kmeans_sums_csr_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *out) {
+cudaError_t kmeans_sums_csr_launch(const KmeansArgs &a, int elem_bytes, int sm_count, double *out, int sums_mode) {
   if (a.rows <= 0) return cudaSuccess;
   if (elem_bytes != 4 && elem_bytes != 8) return cudaErrorInvalidValue;
-  auto kern = elem_bytes == 8 ? kmeans_sums_csr_kernel<double> : kmeans_sums_csr_kernel<float>;
+  if (sums_mode != kKmResidual && sums_mode != kKmNegatives) return cudaErrorInvalidValue;
+  auto kern = sums_mode == kKmNegatives
+                  ? (elem_bytes == 8 ? kmeans_sums_csr_kernel<double, kKmNegatives> : kmeans_sums_csr_kernel<float, kKmNegatives>)
+                  : (elem_bytes == 8 ? kmeans_sums_csr_kernel<double, kKmResidual> : kmeans_sums_csr_kernel<float, kKmResidual>);
   unsigned grid = 0;
   cudaError_t e = warp_grid(kern, a.rows, sm_count, &grid);
   if (e != cudaSuccess) return e;

@@ -1,4 +1,5 @@
-"""org.apache.spark.mllib.evaluation.BinaryClassificationMetrics [mllib-1.3.0] over the shards already in HBM.
+"""org.apache.spark.mllib.evaluation.BinaryClassificationMetrics and MulticlassMetrics [mllib-1.3.0] over the shards already in
+HBM.
 
 The curve is computed on the device (agd_binary_curve): one point per distinct margin of the rows of a view, over every shard
 of the world, in descending order, with exact cumulative counts of true and false positives.  This module derives MLlib's
@@ -10,6 +11,14 @@ Deviations from MLlib, on purpose:
   * with numBins > 0 the points are grouped globally (MLlib groups within each partition): groups of distinct // numBins
     consecutive points, each taking its first (highest) score and the counts at its end;
   * a row whose margin is NaN is not ranked: the constructor raises ValueError when there is one.
+
+MulticlassMetrics follows MLlib's formulas over one confusion matrix (rows: actual labels, columns: predicted, over the distinct
+actual labels, ascending) and the count of each label; on the device both come from agd_label_classes and agd_linear_confusion.
+Deviations from MLlib, on purpose:
+  * labels are compared by value: -0.0 is read as 0.0 (MLlib's maps key -0.0 and 0.0 apart);
+  * the weighted metrics add their terms in ascending label order (MLlib: hash-map order);
+  * a NaN label raises ValueError; a label that is not one of `labels` raises ValueError where MLlib raises
+    NoSuchElementException.
 """
 from __future__ import annotations
 
@@ -113,3 +122,130 @@ class BinaryClassificationMetrics:
         with np.errstate(divide="ignore", invalid="ignore"):
             f = np.where(p + r == 0, 0.0, (1.0 + b2) * (p * r / (b2 * p + r)))
         return np.stack([self.thresholds(), f], axis=1)
+
+
+class MulticlassMetrics:
+    """MulticlassMetrics(predictionAndLabels): from a host (n, 2) array of (prediction, label) rows.
+    MulticlassMetrics(model, data): from a NaiveBayesModel's predictions on the rows of a DeviceDataset or view, over every
+    shard of the world (collective: every rank constructs it with the same arguments and gets the same bits).  A prediction
+    that is none of the labels is a false positive of no label in `labels`, as in MLlib."""
+
+    def __init__(self, *args):
+        if len(args) == 1:
+            labels, counts, confusion = self._host(args[0])
+        elif len(args) == 2:
+            labels, counts, confusion = self._device(*args)
+        else:
+            raise TypeError("MulticlassMetrics(predictionAndLabels) or MulticlassMetrics(model, data)")
+        self.labels = labels
+        self._count = counts.astype(np.float64)
+        self._n = float(counts.sum())
+        self.confusionMatrix = confusion
+        self._tp = np.diagonal(confusion).copy()
+        self._fp = confusion.sum(axis=0) - self._tp   # column sums of integers: exact
+
+    @staticmethod
+    def _host(predictionAndLabels):
+        pl = np.asarray(predictionAndLabels, dtype=np.float64)
+        if pl.ndim != 2 or pl.shape[1] != 2:
+            raise ValueError(f"predictionAndLabels must be an (n, 2) array, got shape {pl.shape}")
+        pred, lab = pl[:, 0] + 0.0, pl[:, 1] + 0.0
+        if np.isnan(lab).any():
+            raise ValueError(f"{int(np.isnan(lab).sum())} rows have a NaN label")
+        labels, li, counts = np.unique(lab, return_inverse=True, return_counts=True)
+        L = labels.shape[0]
+        pj = np.searchsorted(labels, pred) if L else np.zeros(pred.shape[0], dtype=np.int64)
+        hit = (pj < L) & (labels[np.minimum(pj, max(L - 1, 0))] == pred) if L else np.zeros(pred.shape[0], dtype=bool)
+        confusion = np.zeros((L, L), dtype=np.float64)
+        np.add.at(confusion, (li[hit], pj[hit]), 1.0)
+        return labels, counts.astype(np.int64), confusion
+
+    @staticmethod
+    def _device(model, data):
+        labels, counts, nan = data.label_classes()
+        if nan:
+            raise ValueError(f"{nan} rows of the data have a NaN label")
+        L = labels.shape[0]
+        confusion = np.zeros((L, L), dtype=np.float64)
+        if L == 0:
+            return labels, counts, confusion
+        if L > N.MAX_CLASSES:
+            raise ValueError(f"{L} distinct labels, more than the {N.MAX_CLASSES} classes MulticlassMetrics takes on the device")
+        W, b = model._device_model()
+        cnt = data.linear_confusion(W, b, labels)                 # (L, C) by the model's class index
+        cols = np.searchsorted(labels, model.labels)
+        for c in range(model.labels.shape[0]):                    # a model class that is no data label counts nowhere
+            j = int(cols[c])
+            if j < L and labels[j] == model.labels[c]:
+                confusion[:, j] += cnt[:, c]
+        return labels, counts, confusion
+
+    def _index(self, label) -> int:
+        v = float(label) + 0.0
+        j = int(np.searchsorted(self.labels, v))
+        if j >= self.labels.shape[0] or self.labels[j] != v:
+            raise ValueError(f"{label} is not one of the labels")
+        return j
+
+    def truePositiveRate(self, label) -> float:
+        return self.recall(label)
+
+    def _fpr(self, j: int) -> float:
+        with np.errstate(divide="ignore", invalid="ignore"):   # a single label: 0 / 0, NaN as in MLlib
+            return self._fp[j] / np.float64(self._n - self._count[j])
+
+    def falsePositiveRate(self, label) -> float:
+        return self._fpr(self._index(label))
+
+    def _precision(self, j: int) -> float:
+        tp, fp = self._tp[j], self._fp[j]
+        return 0.0 if tp + fp == 0 else tp / (tp + fp)
+
+    def _recall(self, j: int) -> float:
+        return self._tp[j] / self._count[j]
+
+    def _f(self, j: int, beta: float) -> float:
+        p, r = self._precision(j), self._recall(j)
+        b2 = float(beta) * float(beta)
+        return 0.0 if p + r == 0 else (1.0 + b2) * p * r / (b2 * p + r)
+
+    def _weighted(self, metric) -> float:
+        total = 0.0
+        for j in range(self.labels.shape[0]):
+            total += metric(j) * self._count[j] / self._n
+        return total
+
+    def precision(self, label=None) -> float:
+        """precision(label), or with no label the overall precision (the fraction of rows predicted right)."""
+        if label is None:
+            return float(self._tp.sum()) / self._n if self._n else float("nan")
+        return self._precision(self._index(label))
+
+    def recall(self, label=None) -> float:
+        if label is None:
+            return self.precision()
+        return self._recall(self._index(label))
+
+    def fMeasure(self, label=None, beta: float = 1.0) -> float:
+        if label is None:
+            return self.precision()
+        return self._f(self._index(label), beta)
+
+    @property
+    def weightedTruePositiveRate(self) -> float:
+        return self.weightedRecall
+
+    @property
+    def weightedFalsePositiveRate(self) -> float:
+        return self._weighted(self._fpr)
+
+    @property
+    def weightedRecall(self) -> float:
+        return self._weighted(self._recall)
+
+    @property
+    def weightedPrecision(self) -> float:
+        return self._weighted(self._precision)
+
+    def weightedFMeasure(self, beta: float = 1.0) -> float:
+        return self._weighted(lambda j: self._f(j, beta))

@@ -657,6 +657,80 @@ class DeviceDataset:
             dists.append(dist[keep])
         return np.concatenate(cls), np.concatenate(dists)
 
+    # classification (agd_label_classes / agd_class_sums / agd_linear_*): labels compared by value, features in this dataset's
+    # (or view's) space, d = self.d columns, transform applied on the device
+    def _linear(self, W, offset):
+        W = np.ascontiguousarray(W, dtype=np.float64)
+        if W.ndim != 2 or W.shape[0] < 1 or W.shape[1] != self.d:
+            raise ValueError(f"W has shape {W.shape}, data has {self.d} features")
+        b = np.ascontiguousarray(offset, dtype=np.float64)
+        if b.shape != (W.shape[0],):
+            raise ValueError(f"offset has shape {b.shape}, W has {W.shape[0]} rows")
+        return W, b
+
+    @staticmethod
+    def _classes(labels) -> np.ndarray:
+        c = np.ascontiguousarray(labels, dtype=np.float64)
+        if c.ndim != 1:
+            raise ValueError(f"labels must be a vector, got shape {c.shape}")
+        return c + 0.0   # -0.0 -> 0.0
+
+    def label_classes(self):
+        """The distinct labels of the rows over every shard of the world (agd_label_classes; collective: every rank gets the
+        same values): (labels ascending, their counts (int64), rows whose label is NaN).  -0.0 is counted as 0.0."""
+        L = N.lib()
+        n, nan = C.c_int64(), C.c_int64()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(L.agd_label_classes(self.h, 0, None, None, C.byref(n), C.byref(nan)), self.h)
+            labels, counts = np.empty(n.value, dtype=np.float64), np.empty(n.value, dtype=np.int64)
+            if n.value:
+                N.check(L.agd_label_classes(self.h, n.value, _ptr(labels), _ptr(counts), C.byref(n), C.byref(nan)), self.h)
+        return labels, counts, int(nan.value)
+
+    def class_sums(self, labels):
+        """Per class label (ascending, distinct, not NaN) over every shard of the world (agd_class_sums; collective):
+        (sums (C, d) of the features of the rows with that label, their counts, entries of those rows that are not >= 0)."""
+        c = self._classes(labels)
+        sums = np.empty((c.shape[0], self.d), dtype=np.float64)
+        counts = np.empty(c.shape[0], dtype=np.float64)
+        neg = C.c_double()
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(N.lib().agd_class_sums(self.h, _ptr(c), c.shape[0], _ptr(sums), _ptr(counts), C.byref(neg)), self.h)
+        return sums, counts, int(neg.value)
+
+    def linear_argmax_rows(self, dev: int, row0: int, rows: int, W, offset) -> np.ndarray:
+        """The lowest c maximising offset_c + x . W_c (-1 outside the view) of physical rows [row0, row0 + rows) of local
+        device `dev`'s shard (agd_linear_argmax; not collective)."""
+        W, b = self._linear(W, offset)
+        cl = np.empty(max(int(rows), 0), dtype=np.int32)
+        with self._filtered():
+            N.check(N.lib().agd_linear_argmax(self.h, dev, _ptr(W), W.shape[0], _ptr(b), int(row0), int(rows), _ptr(cl)),
+                    self.h)
+        return cl
+
+    def linear_argmax(self, W, offset) -> np.ndarray:
+        """The argmax class of this process's rows, across its local devices in load order (not collective); on a view, of
+        the view's rows only, in the same order as margins."""
+        parts = []
+        for i in range(len(self.ctx.devices)):
+            cl = self.linear_argmax_rows(i, 0, self.local_rows(i), W, offset)
+            parts.append(cl[cl >= 0])
+        return np.concatenate(parts)
+
+    def linear_confusion(self, W, offset, labels) -> np.ndarray:
+        """(L, C) exact counts of the rows over every shard of the world (agd_linear_confusion; collective) by (index of
+        their label in `labels`, argmax class); rows whose label is none of `labels` are not counted."""
+        W, b = self._linear(W, offset)
+        c = self._classes(labels)
+        out = np.empty((c.shape[0], W.shape[0]), dtype=np.float64)
+        self._ensure_exchange()
+        with self._filtered():
+            N.check(N.lib().agd_linear_confusion(self.h, _ptr(W), W.shape[0], _ptr(b), _ptr(c), c.shape[0], _ptr(out)),
+                    self.h)
+        return out
+
     def prox(self, updater: Updater, w, g, step: float, reg: float):
         """applyProjector (AGD.scala:214-222): (regVal, newWeights)."""
         w = np.ascontiguousarray(w, dtype=np.float64)
